@@ -3,7 +3,7 @@
 
 Workloads (`--workload`, named in config.workload; default = north_star's headline):
   tsp100  TSP-100 AttentionModel greedy rollout, 65 536 instances PER GPU (weak scaling, BASELINE metric
-          "node-selections/sec TSP-100 AM rollout @1/2/4/8 B200")
+          "node-selections/sec TSP-100 AM rollout @1/2/4/8 H100")
   c2      TSP-50 greedy, 4 096 instances per GPU            (BASELINE configs[1])
   c3      CVRP-50 sampling (in-kernel Philox), 4 096 per GPU (BASELINE configs[2])
   c4      TSP-100 POMO: 1 024 instances IN TOTAL x 8 dihedral augmentations x 100 starts, 6-layer
@@ -13,7 +13,7 @@ Workloads (`--workload`, named in config.workload; default = north_star's headli
           Adam, mean baseline over the GLOBAL batch through one {sum,count} all-reduce
 
   value : the step with inputs RESIDENT in HBM.
-          rollout workloads: FusedAttentionModelDecoder._precompute_cache (one tcgen05 3xTF32 GEMM) + co_rollout
+          rollout workloads: FusedAttentionModelDecoder._precompute_cache (one wgmma 3xTF32 GEMM) + co_rollout
           (persistent kernel: context + glimpse + pointer + tanh/mask/log-softmax + selection + env step +
           incremental tour length, all T steps) from the resident encoder output;
           c4: cache GEMM + query-batched co_rollout (100 starts share K/V/L) + POMO max reductions;
@@ -25,8 +25,12 @@ Workloads (`--workload`, named in config.workload; default = north_star's headli
 
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.  The
 resident inputs of the default workload (13.4 GB cache + 3.4 GB embeddings per rank) are far larger than the
-126 MB L2, so no explicit L2 flush is needed between iterations (stated in config).  Outside the timed region a
-parity gate re-checks a 1 024-row slice of the timed batch against the CPU oracle (`parity_gate` in the line).
+50 MB L2 of an H100, so no explicit L2 flush is needed between iterations (stated in config).  Outside the timed
+region a parity gate re-checks a 1 024-row slice of the timed batch against the CPU oracle (`parity_gate` in the line).
+
+`--dump-outputs DIR` writes what the last timed value step returned (actions, log-probabilities, reward, ...) as
+DIR/<name>.npy, float32 (float64 for float64 tensors), at most 64 MB in all: an output too large for its share is cut
+down to a fixed, seeded sample of its rows.  Inputs and weights are seeded, so two builds can be compared array by array.
 """
 
 from __future__ import annotations
@@ -75,7 +79,12 @@ def parse():
     p.add_argument("--no-cpu-baseline", action="store_true")
     p.add_argument("--no-e2e", action="store_true")
     p.add_argument("--no-parity-gate", action="store_true")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write the outputs of the last timed value step as DIR/<name>.npy (at most 64 MB in all)")
+    args = p.parse_args()
+    if args.steps < 1:
+        p.error("--steps must be at least 1")
+    return args
 
 
 # ------------------------------------------------------------------------------------ clocks
@@ -147,27 +156,32 @@ def algorithmic_bytes_per_instance(env_name, N, T, S=1):
     return b
 
 
-def measured_peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return json.load(f)["hbm_gbs"], "measured"
-    except Exception:
-        return 6650.0, "fallback"
+#: HBM3 bandwidth of the H100 SXM in GB/s (NVIDIA data sheet); the roofline's denominator, not a measured figure
+HBM_PEAK_GBS = 3350.0
+
+DUMP_BUDGET_BYTES = 64 << 20
 
 
-def ncu_traffic(workload, instances):
-    """dram__bytes_read+write of the dominant kernel from the committed `ncu --set full` capture, per instance,
-    scaled to this launch (the kernel streams each instance exactly once)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "rollout_traffic.json")) as f:
-            d = json.load(f)
-        if workload in d:
-            return d[workload]["dram_bytes_per_instance"] * instances
-        if workload == "tsp100" and "dram_bytes_per_instance" in d:
-            return d["dram_bytes_per_instance"] * instances
-    except Exception:
-        pass
-    return None
+def dump_outputs(directory, res):
+    """Write every tensor the value step returned as <directory>/<name>.npy: the results a caller uses (actions,
+    logprobs, reward, log_likelihood, ...) and the step counters that come with them (steps, max_steps).  Integer
+    tensors are stored as float32, which is exact for node indices and step counts (far below 2^24).  Every array gets
+    an equal share of the 64 MB budget; a larger one keeps a seeded sample of its rows (the same rows in every run), in
+    ascending row order."""
+    import numpy as np
+
+    tensors = {k: v for k, v in res.items() if isinstance(v, torch.Tensor) and v.numel() > 0}
+    os.makedirs(directory, exist_ok=True)
+    share = DUMP_BUDGET_BYTES // max(1, len(tensors))
+    for name, t in sorted(tensors.items()):
+        t = t.detach().to("cpu", torch.float64 if t.dtype == torch.float64 else torch.float32)
+        t = t.reshape(1) if t.dim() == 0 else t
+        row_bytes = max(1, t[0].numel()) * t.element_size()
+        if t.shape[0] * row_bytes > share:
+            gen = torch.Generator().manual_seed(0)
+            rows = torch.randperm(t.shape[0], generator=gen)[: max(1, share // row_bytes)].sort().values
+            t = t[rows]
+        np.save(os.path.join(directory, name + ".npy"), t.contiguous().numpy())
 
 
 # ------------------------------------------------------------------------------------ CPU arm
@@ -304,8 +318,7 @@ def run_ours(args, wl):
 
     def baseline_allreduce(reward):
         """REINFORCE mean baseline over the GLOBAL batch: {sum, count} in f64 (north_star).  The next step does
-        not depend on it, so the NCCL all-reduce runs on a side stream and overlaps the next step's kernels
-        (round 1 had it stream-serialised behind every rollout: every rank waited for the slowest rank)."""
+        not depend on it, so the NCCL all-reduce runs on a side stream and overlaps the next step's kernels."""
         stats.zero_()
         native.reward_stats(reward, stats)
         if world > 1:
@@ -513,22 +526,23 @@ def run_ours(args, wl):
             dist.destroy_process_group()
         return
 
-    peak, peak_kind = measured_peaks()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, res)
+
+    sm_count = native.lib().co_device_sm_count()
     inst_kernel = B * (8 if kind == "pomo" else 1)
     T_avg = sel_per_step_rank / (inst_kernel * S_kernel)
     roofline = None
     if kind != "train":
         bytes_per_launch = algorithmic_bytes_per_instance(env_name, N, T_avg, S_kernel) * inst_kernel
         achieved = bytes_per_launch / (k_ms_avg * 1e-3) / 1e9
-        roofline = {"bound": "hbm", "kernel": kernel_name, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                    "frac": achieved / peak, "peak_source": f"{peak_kind} (MEASURED_PEAKS.json hbm_gbs)",
-                    "traffic": ncu_traffic(args.workload, inst_kernel), "kernel_ms": k_ms_avg,
+        roofline = {"bound": "hbm", "kernel": kernel_name, "achieved": achieved, "peak": HBM_PEAK_GBS, "unit": "GB/s",
+                    "frac": achieved / HBM_PEAK_GBS, "peak_source": "H100 SXM data sheet (HBM3)", "kernel_ms": k_ms_avg,
                     "algorithmic_bytes_per_launch": bytes_per_launch,
                     "kernel_share_of_step": k_ms_avg * args.steps / ms_total,
-                    "cycles_per_selection_per_sm": (k_ms_avg * 1e-3 * (clocks["sm_mhz"] or 1965.0) * 1e6 * 148
-                                                    / sel_per_step_rank) if clocks else None,
-                    "note": "latency/issue-bound on-chip loop (one instance per SM); HBM roofline shown as required, "
-                            "see DESIGN.md 4.1"}
+                    "cycles_per_selection_per_sm": (k_ms_avg * 1e-3 * clocks["sm_mhz"] * 1e6 * sm_count
+                                                    / sel_per_step_rank) if clocks and clocks["sm_mhz"] else None,
+                    "note": "latency/issue-bound on-chip loop (one instance per SM); HBM roofline shown for scale"}
 
     cpu_baseline = None
     if world == 1 and not args.no_cpu_baseline:
@@ -539,6 +553,7 @@ def run_ours(args, wl):
             cpu_baseline = {"value": None, "unit": UNIT, "cores": 0, "kind": "unavailable", "sample": repr(exc)}
 
     line = {
+        "device": torch.cuda.get_device_name(dev),
         "metric": wl["metric"], "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
         "warmup": max(args.warmup, 3), "ms_per_step": ms_total / args.steps, "higher_is_better": True,
         "scaling": "weak" if wl["per_gpu"] else "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -547,9 +562,9 @@ def run_ours(args, wl):
                    "parallelism": f"dp{world} (instances sharded, no data-path collective; "
                                   + ("baseline {sum,count} + gradient all-reduce" if kind == "train" else "baseline {sum,count} all-reduce on a side stream") + ")",
                    "value_scope": scope,
-                   "l2_policy": "resident inputs per rank exceed the 126 MB L2; no flush needed",
+                   "l2_policy": "resident inputs per rank exceed the 50 MB L2; no flush needed",
                    "policy": f"AttentionModelPolicy E=128 H=8 {policy_kwargs(wl)} random-init seed 0"},
-        "clocks": clocks, "e2e": e2e, "gpu_launches": n_launch, "roofline": roofline, "cpu_baseline": cpu_baseline,
+        "peak_allocated_gb": torch.cuda.max_memory_allocated(dev) / 1e9, "clocks": clocks, "e2e": e2e, "gpu_launches": n_launch, "roofline": roofline, "cpu_baseline": cpu_baseline,
         "selections_per_step": sel_total_per_step, "parity_gate": gate,
     }
     if kind == "train":

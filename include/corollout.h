@@ -1,5 +1,5 @@
 /*
- * corollout.h -- C ABI of libcorollout.so, the B200 (sm_100a) rollout engine behind
+ * corollout.h -- C ABI of libcorollout.so, the H100 (sm_90a) rollout engine behind
  * rl4co's env / decoder API.
  *
  * The reference (ai4co/rl4co) is 100% Python and has no FFI on this path; its only FFI
@@ -225,7 +225,7 @@ typedef struct co_rollout_args {
   int32_t* steps_out;        /* [B_traj]  decode steps until done (incl. forced start) */
   int32_t* max_steps_out;    /* [1] device int32, caller-zeroed: max over trajectories */
   float* used_capacity_out;  /* [B_traj] final used capacity (cvrp) or NULL            */
-  /* round 2: narrow tsp cache (no first-node table) -- the first-node half of project_context
+  /* narrow tsp cache (no first-node table) -- the first-node half of project_context
    * (context.py:129-133) becomes one 128x128 GEMV per episode inside the kernel            */
   const float* node_emb;     /* [B_inst, N, E] encoder output; tsp with cache_width 4E  */
   const float* w_first;      /* [E, E] = project_context.weight[:, :E] row-major; same   */
@@ -248,7 +248,7 @@ int co_rollout(const co_rollout_args* args, void* stream);
 
 /* ------------------------------------------------------------------ dense projections
  *
- * fp32-accurate GEMM on tcgen05 tensor cores (kind::tf32, 3xTF32 hi/lo split, fp32 TMEM
+ * fp32-accurate GEMM on wgmma tensor cores (kind tf32, 3xTF32 hi/lo split, fp32 register
  * accumulators):  C[M,Nout] = epilogue(A[M,K] @ W[Nout,K]^T),
  *   epilogue(v) = relu?((v + bias[n]) + residual[m,n]) * scale[n] + shift[n]   (each optional)
  * Replaces the nn.Linear calls of AttentionModelDecoder._precompute_cache

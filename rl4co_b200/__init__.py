@@ -1,4 +1,4 @@
-"""rl4co_b200 -- B200 (sm_100a) rollout engine behind rl4co's env / decoder API.
+"""rl4co_b200 -- H100 (sm_90a) rollout engine behind rl4co's env / decoder API.
 
 Scope: the autoregressive construction hot path only (SURVEY.md section 8):
   envs      FusedTSPEnv, FusedCVRPEnv          <- rl4co.envs.TSPEnv / CVRPEnv

@@ -4,8 +4,7 @@
   encoder self-attention under autograd     rl4co/models/nn/attention.py:110-134  (F.scaled_dot_product_attention)
   glimpse of the teacher-forced pass        rl4co/models/nn/attention.py:300-314, models/zoo/am/decoder.py:156-193
 
-`F.scaled_dot_product_attention` in fp32 is what the reference runs here; on the B200 its mem-efficient kernels took
-75 ms of the 151 ms CVRP-100 training chunk.  The functions below are autograd.Function wrappers: forward saves the
+`F.scaled_dot_product_attention` in fp32 is what the reference runs here.  The functions below are autograd.Function wrappers: forward saves the
 per-row log-sum-exp, backward recomputes the probabilities (no N x N tensor in memory).  CUDA only -- there is no
 fallback inside this module; callers decide (shape limits: 8 heads x 16, keys <= 128, queries <= 256 per call).
 """

@@ -5,15 +5,14 @@
 //   * the glimpse of the teacher-forced log-likelihood pass: all T decode steps of an instance are T independent
 //     queries against its cached K / V with the replayed action mask (models/zoo/am/decoder.py:156-193,
 //     nn/attention.py:300-314; Evaluate decoding utils/decoding.py:448-461)
-// replacing torch's mem-efficient SDPA (fp32 fmha_cutlassF/B 64x64: 5.5 ms forward, 13 ms backward per call at
-// 8 192 x 101, 75 ms of the 151 ms CVRP-100 training chunk -- profiles/r02_train_step_profile.txt).
+// replacing torch's mem-efficient SDPA (fp32 fmha_cutlassF/B 64x64).
 //
 // Design: head dimension 16 makes this a SIMT fp32 problem (a 16-deep contraction per score): one CTA per
 // (instance, head); K_h / V_h (forward, dQ) or Q_h / dO_h (dK, dV) staged once in shared memory and read as
 // warp-uniform LDS.128 broadcasts; every thread owns TWO query rows (or two keys) so that each broadcast feeds two
-// packed-FFMA2 chains (one row per thread would be bound by the 2-cycle LDS.128 broadcast, not by the FMA pipe).
+// float2 FMA chains (one row per thread would be bound by the 2-cycle LDS.128 broadcast, not by the FMA pipe).
 // No N x N matrix ever exists in memory: the backward recomputes the probabilities from the saved log-sum-exp.
-//   forward: two passes over the keys (row max, then exp / accumulate): exact softmax, 24 FFMA2 per (row, key)
+//   forward: two passes over the keys (row max, then exp / accumulate): exact softmax, 24 FMA pairs per (row, key)
 //   dQ     : thread = 2 query rows;  dS = P o (dO V^T - rowsum(dO o O));  dQ = scale * dS K
 //   dK, dV : thread = 2 keys;        dK = scale * dS^T Q,  dV = P^T dO      (no atomics, no cross-thread reduction)
 // Masks come bit-packed: 4 x uint32 per query row (bit n of word n / 32 set = key n may be attended).
@@ -25,7 +24,6 @@ namespace attn {
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
 
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
 __device__ __forceinline__ float ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

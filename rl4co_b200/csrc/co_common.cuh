@@ -1,4 +1,4 @@
-// Shared helpers for libcorollout (sm_100a). See include/corollout.h for the ABI.
+// Shared helpers for libcorollout (sm_90a). See include/corollout.h for the ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -46,6 +46,11 @@ struct PerDeviceOnce {
     return done[dev & 63];
   }
 };
+
+// two independent fp32 FMAs / multiplies on a float2 (Hopper has no packed fp32 instruction; results are the same
+// round-to-nearest values per component)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

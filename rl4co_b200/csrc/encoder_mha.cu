@@ -7,8 +7,8 @@
 // One CTA per instance, warp h = head h.  K and V of the instance (all heads) are staged once in
 // shared memory; lane l owns query rows l, l+32, .. (ROWS per lane) with q and the output
 // accumulators in registers.  Keys are consumed four at a time with an online (flash-style)
-// softmax: scores via packed FFMA2, one rescale per block, ex2.approx, value accumulation via
-// FFMA2.  No N x N matrix ever exists in memory: HBM traffic = read qkv once + write out once
+// softmax: scores via float2 FMA pairs, one rescale per block, ex2.approx, value accumulation via
+// float2 FMA pairs.  No N x N matrix ever exists in memory: HBM traffic = read qkv once + write out once
 // (N*(384+128)*4 B per instance).
 #include <stdlib.h>
 #include <string.h>
@@ -17,8 +17,6 @@
 
 namespace co {
 
-__device__ __forceinline__ float2 ffma2_(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-__device__ __forceinline__ float2 fmul2_(float2 a, float2 b) { return __fmul2_rn(a, b); }
 __device__ __forceinline__ float ex2_(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -70,14 +68,14 @@ __global__ void __launch_bounds__(256 * WPH, (ROWS * WPH == 4) ? 1 : 2) encoder_
         const float4 k0 = kp[0], k1 = kp[1], k2 = kp[2], k3 = kp[3];
 #pragma unroll
         for (int r = 0; r < ROWS; ++r) {
-          float2 a = fmul2_(q[r][0], make_float2(k0.x, k0.y));
-          a = ffma2_(q[r][1], make_float2(k0.z, k0.w), a);
-          a = ffma2_(q[r][2], make_float2(k1.x, k1.y), a);
-          a = ffma2_(q[r][3], make_float2(k1.z, k1.w), a);
-          float2 c = fmul2_(q[r][4], make_float2(k2.x, k2.y));
-          c = ffma2_(q[r][5], make_float2(k2.z, k2.w), c);
-          c = ffma2_(q[r][6], make_float2(k3.x, k3.y), c);
-          c = ffma2_(q[r][7], make_float2(k3.z, k3.w), c);
+          float2 a = fmul2(q[r][0], make_float2(k0.x, k0.y));
+          a = ffma2(q[r][1], make_float2(k0.z, k0.w), a);
+          a = ffma2(q[r][2], make_float2(k1.x, k1.y), a);
+          a = ffma2(q[r][3], make_float2(k1.z, k1.w), a);
+          float2 c = fmul2(q[r][4], make_float2(k2.x, k2.y));
+          c = ffma2(q[r][5], make_float2(k2.z, k2.w), c);
+          c = ffma2(q[r][6], make_float2(k3.x, k3.y), c);
+          c = ffma2(q[r][7], make_float2(k3.z, k3.w), c);
           s[r][jj] = (j0 + jj < N) ? (a.x + a.y) + (c.x + c.y) : -INFINITY;
         }
       }
@@ -92,7 +90,7 @@ __global__ void __launch_bounds__(256 * WPH, (ROWS * WPH == 4) ? 1 : 2) encoder_
         l[r] = fmaf(l[r], corr, (p[r][0] + p[r][1]) + (p[r][2] + p[r][3]));
         const float2 c2 = make_float2(corr, corr);
 #pragma unroll
-        for (int c = 0; c < 8; ++c) o[r][c] = fmul2_(o[r][c], c2);
+        for (int c = 0; c < 8; ++c) o[r][c] = fmul2(o[r][c], c2);
       }
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) {
@@ -102,14 +100,14 @@ __global__ void __launch_bounds__(256 * WPH, (ROWS * WPH == 4) ? 1 : 2) encoder_
 #pragma unroll
         for (int r = 0; r < ROWS; ++r) {
           const float2 pp = make_float2(p[r][jj], p[r][jj]);
-          o[r][0] = ffma2_(pp, make_float2(v0.x, v0.y), o[r][0]);
-          o[r][1] = ffma2_(pp, make_float2(v0.z, v0.w), o[r][1]);
-          o[r][2] = ffma2_(pp, make_float2(v1.x, v1.y), o[r][2]);
-          o[r][3] = ffma2_(pp, make_float2(v1.z, v1.w), o[r][3]);
-          o[r][4] = ffma2_(pp, make_float2(v2.x, v2.y), o[r][4]);
-          o[r][5] = ffma2_(pp, make_float2(v2.z, v2.w), o[r][5]);
-          o[r][6] = ffma2_(pp, make_float2(v3.x, v3.y), o[r][6]);
-          o[r][7] = ffma2_(pp, make_float2(v3.z, v3.w), o[r][7]);
+          o[r][0] = ffma2(pp, make_float2(v0.x, v0.y), o[r][0]);
+          o[r][1] = ffma2(pp, make_float2(v0.z, v0.w), o[r][1]);
+          o[r][2] = ffma2(pp, make_float2(v1.x, v1.y), o[r][2]);
+          o[r][3] = ffma2(pp, make_float2(v1.z, v1.w), o[r][3]);
+          o[r][4] = ffma2(pp, make_float2(v2.x, v2.y), o[r][4]);
+          o[r][5] = ffma2(pp, make_float2(v2.z, v2.w), o[r][5]);
+          o[r][6] = ffma2(pp, make_float2(v3.x, v3.y), o[r][6]);
+          o[r][7] = ffma2(pp, make_float2(v3.z, v3.w), o[r][7]);
         }
       }
     }
@@ -146,9 +144,7 @@ static int launch_mha(const float* qkv, float* out, int B, int N, cudaStream_t s
   return check_launch("co_encoder_mha");
 }
 
-int launch_encoder_mha_tc(const float* qkv, float* out, int B, int N, cudaStream_t stream);   // encoder_mha_tc.cu
-int launch_encoder_mha_tc2(const float* qkv, float* out, int B, int N, cudaStream_t stream);  // encoder_mha_tc2.cu
-int launch_encoder_mha_tc3(const float* qkv, float* out, int B, int N, cudaStream_t stream);  // encoder_mha_tc3.cu
+int launch_encoder_mha_wgmma(const float* qkv, float* out, int B, int N, cudaStream_t stream);  // encoder_mha_wgmma.cu
 
 }  // namespace co
 
@@ -161,14 +157,11 @@ extern "C" int co_encoder_mha(const float* qkv, float* out, int B, int N, void* 
   if (((uintptr_t)qkv | (uintptr_t)out) & 15) return fail(CO_ERR_BAD_ARG, "co_encoder_mha: pointers must be 16-byte aligned%s");
   if (B == 0) return CO_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  // CO_MHA_VARIANT = simt | tc | tc2 | tc3 forces one kernel (read per call so tests can switch); default: tc3
-  // (scores AND P.V on the tensor core, P through TMEM) for N > 64, all-SIMT below (a 128 x 128 score tile is mostly
-  // padding there).
+  // CO_MHA_VARIANT = simt | wgmma forces one kernel (read per call so tests can switch); default: wgmma (scores AND
+  // P.V on the tensor core, P in registers) for N > 64, all-SIMT below (a 128 x 128 score tile is mostly padding there).
   const char* ev = getenv("CO_MHA_VARIANT");
-  if (ev && !strcmp(ev, "tc2")) return launch_encoder_mha_tc2(qkv, out, B, N, st);
-  if (ev && !strcmp(ev, "tc")) return launch_encoder_mha_tc(qkv, out, B, N, st);
-  if (ev ? !strcmp(ev, "tc3") : N > 64) return launch_encoder_mha_tc3(qkv, out, B, N, st);
-  if (ev && strcmp(ev, "simt")) return fail(CO_ERR_BAD_ARG, "co_encoder_mha: CO_MHA_VARIANT must be simt, tc, tc2 or tc3%s");
+  if (ev ? !strcmp(ev, "wgmma") : N > 64) return launch_encoder_mha_wgmma(qkv, out, B, N, st);
+  if (ev && strcmp(ev, "simt")) return fail(CO_ERR_BAD_ARG, "co_encoder_mha: CO_MHA_VARIANT must be simt or wgmma%s");
   if (N <= 32) return launch_mha<1, 1>(qkv, out, B, N, st);
   if (N <= 64) return launch_mha<2, 1>(qkv, out, B, N, st);
   return launch_mha<4, 1>(qkv, out, B, N, st);

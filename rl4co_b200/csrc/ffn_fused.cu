@@ -1,32 +1,32 @@
-// Encoder FFN block fused into one kernel: the [M, 512] hidden activation never leaves the SM.
+// Encoder FFN block fused into one kernel: the [M, 512] hidden activation never leaves the register file.
 //
 //   out = ((x + relu(x W1^T + b1) W2^T + b2) * scale + shift      x [M,128], W1 [512,128], W2 [128,512]
 //   (rl4co/models/nn/graph/attnnet.py:33-53: SkipConnection(MLP) followed by eval-mode BatchNorm folded into scale/shift;
 //    rl4co/models/nn/mlp.py:45-60 is the MLP)
 //
-// Per 128-row tile, 3xTF32 everywhere (hi = cvt.rna.tf32, lo = v - hi; products hi.hi + lo.hi + hi.lo):
+// Per 128-row tile, 3xTF32 everywhere (hi = cvt.rna.tf32, lo = v - hi; products hi.hi + lo.hi + hi.lo).  Two consumer
+// warpgroups own 64 rows each; a producer warpgroup feeds them:
 //   x tile  -> hi / lo K-major SWIZZLE_128B operand tiles in SMEM (4 k-blocks, 128 KB), resident for the tile
 //   for each of the 4 hidden chunks j (128 units):
-//     FF1(j): H = x W1_j^T            48 SS-form MMAs 128x128x8 -> TMEM accumulator H[j & 1]
-//     epilogue warps: H + b1 -> relu -> H_hi written back IN PLACE, H_lo beside it (tcgen05.st, lane = row, column = unit)
-//     FF2(j): Y += H W2_j^T           48 TS-form MMAs (A operand from TMEM, tools/micro/ts_mma_check.cu) -> TMEM Y
+//     FF1(j): H = x W1_j^T            48 wgmma m64n128k8 per warpgroup, operands from SMEM, H in 64 accumulator registers
+//     H + b1 -> relu -> H_hi in place, H_lo beside it, still in registers
+//     FF2(j): Y += H W2_j^T           48 wgmma with the A operand from registers: the accumulator fragment of H is the
+//                                     A fragment once W2's k dimension is stored in the k-slot order of wgmma.cuh
 //   Y + b2 + x, BN, store.
-// TMEM: H0 [0,128) H1 [128,256) H_lo [256,384) Y [384,512). W1_j / W2_j k-blocks ([128 x 32] hi + lo = 32 KB) stream from
-// L2 in the fixed order FF1(0) FF1(1) FF2(0) FF1(2) FF2(1) FF1(3) FF2(2) FF2(3), so the epilogue of chunk j runs under
-// the MMAs of FF1(j+1). Per tile: 384 MMAs x 64 cycles = 24.6 k cycles of tensor pipe and 1 MB of weights.
+// W1_j / W2_j k-blocks ([128 x 32] hi + lo = 32 KB) stream from L2 in the order FF1(0) FF2(0) .. FF1(3) FF2(3) through a
+// 3-stage ring; one MMA batch stays in flight while the stage before it is released.  Per tile 1 MB of weights.
 //
 // Weight stream = TMA bulk copies with CLUSTER MULTICAST.  The kernel runs as 2-CTA clusters; the weights are pre-tiled
 // once per weight version (co_ffn_tile_weights) into the exact shared-memory image of the operand tiles (K-major,
 // SWIZZLE_128B), block after block in issue order, so a block is two contiguous 16 KB pieces (hi, lo).  For every block
 // CTA r of the cluster issues ONE `cp.async.bulk ... .multicast::cluster` of piece r that lands in BOTH CTAs' rings and
-// signals both CTAs' "full" mbarriers (complete_tx); a ring stage is reused when the MMAs of BOTH CTAs have retired
-// (tcgen05.commit multicast onto both "empty" barriers).  Each SM therefore pulls 0.5 MB per tile from L2 instead of 1 MB:
-// the cp.async version measured 22 B/clk/SM of L2 traffic = 54 k cycles per tile (10.6 ms per layer at M = 6.55 M), i.e.
-// it was bound by the L2 stream, not by the tensor pipe.
-// Replaces FF1 (5.4 ms) + four split-K FF2 passes (10.3 ms) per layer.
+// signals both CTAs' "full" mbarriers (complete_tx); a ring stage is reused when the consumer warps of BOTH CTAs have
+// arrived on its "empty" barrier (remote mbarrier arrive).  Each SM therefore pulls 0.5 MB per tile from L2 instead of
+// 1 MB.
 #include <stdint.h>
 
 #include "co_common.cuh"
+#include "wgmma.cuh"
 
 namespace co {
 namespace ffn {
@@ -36,30 +36,13 @@ constexpr int TILE_B = 128 * 32 * 4;                         // one [128 x 32] o
 constexpr int OFF_W = 2 * KB * TILE_B;                       // after x hi / lo
 constexpr int WST = 3;                                       // weight ring stages (hi + lo each): 2 blocks in flight
 constexpr int SMEM_B = OFF_W + WST * 2 * TILE_B;             // 229 376 (x 128 KB + 3 x 32 KB)
-constexpr int THREADS = 448;   // warps 0-3 x producers, 4-7 + 10-13 epilogue (two column halves), 8 issuer, 9 weight loader
+constexpr int THREADS = 384;   // warps 0-2 x producers, warp 3 weight loader, warps 4-7 / 8-11 consumers (64 rows each)
+constexpr int X_PRODUCERS = 96, CONSUMER_WARPS = 8;
 constexpr int CLUSTER = 2;                                   // CTAs sharing every weight block
 constexpr int WBLOCK_FLOATS = 2 * 128 * 32;                  // one pre-tiled block: hi image, lo image (32 KB)
-constexpr uint32_t SBO = 1024, COL_HLO = 256, COL_Y = 384;
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
+constexpr int WBLOCKS = 2 * NJ * KB;                         // weight blocks per tile
+constexpr uint32_t SBO = 1024;
 
-__device__ __forceinline__ uint32_t s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ uint64_t desc(uint32_t saddr) {  // K-major SWIZZLE_128B, SBO 1 KB (gemm_tf32x3.cu)
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(SBO >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ void mma_ss(uint32_t d, uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(d), "l"(a), "l"(b), "r"(IDESC), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void mma_ts(uint32_t d, uint32_t a_tmem, uint64_t b, uint32_t acc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-               ::"r"(d), "r"(a_tmem), "l"(b), "r"(IDESC), "r"(acc) : "memory");
-}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -68,10 +51,10 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the barrier at this CTA-relative offset in EVERY CTA of the cluster when all prior MMAs have retired
-__device__ __forceinline__ void commit_multicast(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)((1u << CLUSTER) - 1)) : "memory");
+// arrive on the barrier at this CTA-relative address in CTA `rank` of the cluster
+__device__ __forceinline__ void bar_arrive_cluster(uint32_t bar, uint32_t rank) {
+  asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
+               "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar), "r"(rank) : "memory");
 }
 __device__ __forceinline__ void bar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -82,68 +65,6 @@ __device__ __forceinline__ void bulk_copy_multicast(uint32_t dst, const void* sr
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
       ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "h"((uint16_t)((1u << CLUSTER) - 1)) : "memory");
 }
-__device__ __forceinline__ void commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void bar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done)
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-__device__ __forceinline__ void fence_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ float rna(float v) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-  return __uint_as_float(u);
-}
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-// tcgen05.wait::ld with the destination registers as in/out operands, so no use of them can be scheduled above it
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                 "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]),
-                 "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :: "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-        "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])),
-        "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])),
-        "r"(__float_as_uint(v[11])), "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])),
-        "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])) : "memory");
-}
 
 struct FfnArgs {
   const float *x, *wtiled, *b1, *b2, *scale, *shift;  // wtiled: co_ffn_tile_weights image; scale / shift may be null
@@ -151,243 +72,199 @@ struct FfnArgs {
   int M, ldx, ldo;
 };
 
-// weight block b (0..31) of a tile in issue order; returns {second GEMM?, chunk j, k-block kb}
+// weight block b (0..31) of a tile in issue order FF1(0) FF2(0) FF1(1) ..: {second GEMM?, chunk j, k-block kb}
 struct WBlock { int ff2, j, kb; };
-__device__ __forceinline__ WBlock wblock(int b) {
-  // phases: FF1(0) FF1(1) FF2(0) FF1(2) FF2(1) FF1(3) FF2(2) FF2(3), four k-blocks each
-  const int ph = b >> 2, kb = b & 3;
-  const int ff2 = (0xD4 >> ph) & 1;                   // phases 2, 4, 6, 7
-  const int j = ff2 ? (ph == 7 ? 3 : (ph >> 1) - 1) : (ph < 2 ? ph : (ph + 1) >> 1);
-  return {ff2, j, kb};
-}
+__host__ __device__ __forceinline__ WBlock wblock(int b) { return {(b >> 2) & 1, b >> 3, b & 3}; }
 
 __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS, 1)
     ffn_fused_kernel(const FfnArgs g, int m_tiles) {
   extern __shared__ __align__(1024) unsigned char smem[];
   unsigned char* sX = smem;           // [kb][hi, lo]
   unsigned char* sW = smem + OFF_W;   // [stage][hi, lo]
-  __shared__ __align__(8) uint64_t bars[14];
-  __shared__ uint32_t tmem_base_s;
-  const uint32_t b0 = s32(bars);
-  auto XFULL = [&]() { return b0; };                          // producers: x tile in SMEM                (128)
-  auto XEMPTY = [&]() { return b0 + 8; };                     // FF1(3) retired: x tile reusable          (commit)
+  __shared__ __align__(8) uint64_t bars[2 + 2 * WST];
+  const uint32_t b0 = wg::s32(bars);
+  auto XFULL = [&]() { return b0; };                          // producers: x tile in SMEM                    (96)
+  auto XEMPTY = [&]() { return b0 + 8; };                     // FF1(3) retired: x tile reusable              (256)
   auto WFULL = [&](int s) { return b0 + 8 * (2 + s); };       // weight block landed: 1 arrive + 32 KB of complete_tx
-  auto WEMPTY = [&](int s) { return b0 + 8 * (5 + s); };      // its MMAs retired in BOTH CTAs      (2 multicast commits)
-  auto HFULL = [&](int a) { return b0 + 8 * (8 + a); };       // FF1(j) retired -> epilogue               (commit)
-  auto HPFULL = [&]() { return b0 + 8 * 10; };                // epilogue: H_hi / H_lo of chunk j written (128)
-  auto HFREE = [&]() { return b0 + 8 * 11; };                 // FF2(j) retired: H[j & 1] and H_lo free   (commit)
-  auto YFULL = [&]() { return b0 + 8 * 12; };                 // FF2(3) retired                           (commit)
-  auto YEMPTY = [&]() { return b0 + 8 * 13; };                // epilogue read Y                          (128)
+  auto WEMPTY = [&](int s) { return b0 + 8 * (2 + WST + s); };  // its MMAs retired: consumer warps of BOTH CTAs (16)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(&tmem_base_s)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
-    auto init = [&](uint32_t bar, int cnt) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(cnt)); };
-    init(XFULL(), 128); init(XEMPTY(), 1); init(HPFULL(), 256); init(HFREE(), 1); init(YFULL(), 1); init(YEMPTY(), 256);
-    for (int s = 0; s < WST; ++s) { init(WFULL(s), 1); init(WEMPTY(s), CLUSTER); }
-    for (int s = 0; s < 2; ++s) init(HFULL(s), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;");
+    wg::bar_init(XFULL(), X_PRODUCERS);
+    wg::bar_init(XEMPTY(), 32 * CONSUMER_WARPS);
+    for (int s = 0; s < WST; ++s) { wg::bar_init(WFULL(s), 1); wg::bar_init(WEMPTY(s), CLUSTER * CONSUMER_WARPS); }
+    wg::bar_init_fence();
   }
-  tc_before();
   __syncthreads();
   cluster_sync();  // the peer's barriers are initialised before anything can arrive on them
-  tc_after();
-  const uint32_t tmem = tmem_base_s;
   // both CTAs of a cluster run the same number of tiles (they consume the same weight-block sequence); a tile index
   // beyond m_tiles is a dummy: every row fails `row < M`, so nothing is loaded or stored for it
   const int ntiles = (m_tiles + (int)gridDim.x - 1) / (int)gridDim.x;
 
   if (warp < 4) {
-    // ------------------------------------------------------------------ producers: x tile (fp32 -> tf32 hi / lo split)
-    const int r4 = lane >> 3, c8 = lane & 7;
-    for (int t = 0; t < ntiles; ++t) {
-      const int m0 = (blockIdx.x + t * gridDim.x) * BM;
-      bar_wait(XEMPTY(), (t & 1) ^ 1);
-#pragma unroll
-      for (int kb = 0; kb < KB; ++kb) {
-        float4 a[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {  // a warp instruction fetches 4 complete 128-byte rows of the k-block
-          const int row = m0 + 16 * j + 4 * warp + r4;
-          a[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (row < g.M) a[j] = __ldg(reinterpret_cast<const float4*>(g.x + (size_t)row * g.ldx + kb * 32 + c8 * 4));
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int lrow = 16 * j + 4 * warp + r4;
-          const uint32_t soff = (lrow >> 3) * SBO + (lrow & 7) * 128 + ((c8 ^ (lrow & 7)) << 4);
-          const float4 h = make_float4(rna(a[j].x), rna(a[j].y), rna(a[j].z), rna(a[j].w));
-          *reinterpret_cast<float4*>(sX + (2 * kb) * TILE_B + soff) = h;
-          *reinterpret_cast<float4*>(sX + (2 * kb + 1) * TILE_B + soff) =
-              make_float4(a[j].x - h.x, a[j].y - h.y, a[j].z - h.z, a[j].w - h.w);
-        }
-      }
-      fence_async();
-      bar_arrive(XFULL());
-    }
-  } else if (warp == 8) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      uint32_t wb = 0, hc = 0;  // weight blocks consumed, hidden chunks started (over all tiles)
-      auto gemm_block = [&](bool ts, uint32_t d, uint32_t a_tmem, bool first) {
-        // one k-block (32) = 4 k-steps x {hi.hi, lo.hi, hi.lo}; A = x tiles (SS) or H_hi / H_lo columns (TS)
-        const int st = wb % WST;
-        bar_wait(WFULL(st), (wb / WST) & 1);
-        tc_after();
-        const uint32_t bhi = s32(sW + (2 * st) * TILE_B), blo = bhi + TILE_B;
-        const int kb = wblock(wb & 31).kb;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint32_t off = kk * 32;
-          if (!ts) {
-            const uint32_t ahi = s32(sX + (2 * kb) * TILE_B), alo = ahi + TILE_B;
-            mma_ss(d, desc(ahi + off), desc(bhi + off), !(first && kb == 0 && kk == 0));
-            mma_ss(d, desc(alo + off), desc(bhi + off), 1);
-            mma_ss(d, desc(ahi + off), desc(blo + off), 1);
-          } else {
-            const uint32_t col = kb * 32 + kk * 8;
-            mma_ts(d, a_tmem + col, desc(bhi + off), !(first && kb == 0 && kk == 0));
-            mma_ts(d, tmem + COL_HLO + col, desc(bhi + off), 1);
-            mma_ts(d, a_tmem + col, desc(blo + off), 1);
-          }
-        }
-        commit_multicast(WEMPTY(st));  // frees the stage in BOTH CTAs' rings (each waits for two arrivals)
-        ++wb;
-      };
-      auto ff1 = [&](uint32_t c) {  // c = global chunk counter; accumulator H[c & 1]
-        for (int kb = 0; kb < KB; ++kb) gemm_block(false, tmem + (c & 1) * 128, 0, true);
-        commit(HFULL(c & 1));
-      };
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+    if (warp < 3) {
+      // ---------------------------------------------------------------- producers: x tile (fp32 -> tf32 hi / lo split)
+      // a warp instruction fetches 4 complete 128-byte rows of a k-block; a quarter-warp writes one swizzled row
+      const int r4 = lane >> 3, c8 = lane & 7;
       for (int t = 0; t < ntiles; ++t) {
-        bar_wait(XFULL(), t & 1);
-        tc_after();
-        ff1(hc);
-        for (int j = 0; j < NJ; ++j) {
-          const uint32_t c = hc + j;
-          if (j + 1 < NJ) {
-            // H[(c + 1) & 1] last held chunk c - 1, read by FF2(c - 1): wait until those MMAs retired
-            if (c >= 1) bar_wait(HFREE(), (c - 1) & 1);
-            ff1(c + 1);
-            if (j + 1 == NJ - 1) commit(XEMPTY());
+        const int m0 = (blockIdx.x + t * gridDim.x) * BM;
+        wg::bar_wait(XEMPTY(), (t & 1) ^ 1);
+        for (int rq0 = warp; rq0 < 32; rq0 += 6) {
+#pragma unroll
+          for (int kb = 0; kb < KB; ++kb) {
+            float4 a[2];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const int lrow = 4 * (rq0 + 3 * u) + r4, row = m0 + lrow;
+              a[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+              if (lrow < BM && row < g.M) a[u] = __ldg(reinterpret_cast<const float4*>(g.x + (size_t)row * g.ldx + kb * 32 + c8 * 4));
+            }
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const int lrow = 4 * (rq0 + 3 * u) + r4;
+              if (lrow < BM) {
+                const uint32_t soff = (lrow >> 3) * SBO + (lrow & 7) * 128 + ((c8 ^ (lrow & 7)) << 4);
+                const float4 h = make_float4(wg::rna_tf32(a[u].x), wg::rna_tf32(a[u].y), wg::rna_tf32(a[u].z), wg::rna_tf32(a[u].w));
+                *reinterpret_cast<float4*>(sX + (2 * kb) * TILE_B + soff) = h;
+                *reinterpret_cast<float4*>(sX + (2 * kb + 1) * TILE_B + soff) =
+                    make_float4(a[u].x - h.x, a[u].y - h.y, a[u].z - h.z, a[u].w - h.w);
+              }
+            }
           }
-          bar_wait(HPFULL(), c & 1);
-          // Y of the previous tile must have been read by the epilogue before FF2(0) overwrites it (FF1 of this tile
-          // does not touch Y, so the wait sits here and not at the top of the tile)
-          if (j == 0) bar_wait(YEMPTY(), (t & 1) ^ 1);
-          tc_after();
-          for (int kb = 0; kb < KB; ++kb) gemm_block(true, tmem + COL_Y, tmem + (c & 1) * 128, j == 0);
-          commit(HFREE());
         }
-        commit(YFULL());
-        hc += NJ;
+        wg::fence_async();
+        wg::bar_arrive(XFULL());
       }
-    }
-    __syncwarp();
-  } else if (warp == 9) {
-    // ------------------------------------------------------------------ weight loader: one thread, TMA bulk copies
-    if (lane == 0) {
+    } else if (lane == 0) {
+      // ---------------------------------------------------------------- weight loader: one thread, TMA bulk copies
       const uint32_t rank = cluster_ctarank();
       uint32_t wb = 0;
       for (int t = 0; t < ntiles; ++t) {
-        for (int b = 0; b < 32; ++b, ++wb) {
+        for (int b = 0; b < WBLOCKS; ++b, ++wb) {
           const int st = wb % WST;
-          bar_wait(WEMPTY(st), ((wb / WST) & 1) ^ 1);   // the stage is free in both CTAs
-          bar_expect_tx(WFULL(st), 2 * TILE_B);           // own piece + the peer's piece will land here
+          wg::bar_wait(WEMPTY(st), ((wb / WST) & 1) ^ 1);   // the stage is free in both CTAs
+          bar_expect_tx(WFULL(st), 2 * TILE_B);             // own piece + the peer's piece will land here
           // piece `rank` (0 = hi image, 1 = lo image) of block b -> the same ring slot of every CTA in the cluster
-          bulk_copy_multicast(s32(sW + (2 * st + rank) * TILE_B), g.wtiled + (size_t)b * WBLOCK_FLOATS + rank * (TILE_B / 4),
+          bulk_copy_multicast(wg::s32(sW + (2 * st + rank) * TILE_B), g.wtiled + (size_t)b * WBLOCK_FLOATS + rank * (TILE_B / 4),
                               TILE_B, WFULL(st));
         }
       }
     }
-    __syncwarp();
   } else {
-    // ------------------------------------------------------------------ epilogue warps 4..7: one row per thread
-    // two groups of four warps (4..7 and 10..13), each covering the four TMEM lane quarters (quarter = warp % 4) and
-    // one half of the columns: the per-chunk epilogue has to finish inside one FF1 (3 072 cycles of MMAs)
-    const int q4 = warp & 3, row_in_tile = 32 * q4 + lane, eg = (warp >= 10) ? 1 : 0;
-    const uint32_t lane_base = tmem + ((uint32_t)(32 * q4) << 16);
-    uint32_t c = 0;
-    uint32_t r[32];
+    // ------------------------------------------------------------------ consumer warpgroups: rows [64 cw, 64 cw + 64)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
+    const int cw = (warp - 4) >> 2, w4 = warp & 3, gq = lane >> 2, q = lane & 3;
+    const uint32_t xbase = wg::s32(sX) + cw * 64 * 128;
+    uint32_t wb = 0;   // weight blocks consumed (over all tiles)
+    int held = -1;     // ring stage whose MMA batch is still in flight
+    auto release = [&](int st) {  // this warp's MMAs on stage st have retired: tell the loaders of both CTAs
+      __syncwarp();
+      if (lane == 0)
+        for (uint32_t r = 0; r < CLUSTER; ++r) bar_arrive_cluster(WEMPTY(st), r);
+    };
+    auto committed = [&](int st) {  // a batch on stage st was just committed: the one before it has retired
+      wg::commit();
+      if (held >= 0) { wg::wait<1>(); release(held); }
+      held = st;
+    };
+    auto drain = [&]() {
+      wg::wait<0>();
+      if (held >= 0) release(held);
+      held = -1;
+    };
+    float h[64], y[64];
+    uint32_t hlo[2][4][4];
     for (int t = 0; t < ntiles; ++t) {
-      const int row = (blockIdx.x + t * gridDim.x) * BM + row_in_tile;
-      for (int j = 0; j < NJ; ++j, ++c) {
-        bar_wait(HFULL(c & 1), (c >> 1) & 1);
-        tc_after();
-        const uint32_t hcol = lane_base + (c & 1) * 128;
-        // 32 columns at a time; the TMEM load of the next 32 columns is in flight while the current ones are processed
-        // (bias + ReLU + tf32 split).  The bias comes in 16-byte uniform loads (it was one LDG per element: 128 per
-        // thread and chunk, which made this epilogue -- not the MMAs -- the pacing stage of the kernel).
-        auto process = [&](const uint32_t (&rr)[32], int cc) {
+      const int m0 = (blockIdx.x + t * gridDim.x) * BM + 64 * cw + 16 * w4 + gq;  // this thread's rows: m0, m0 + 8
+      wg::bar_wait(XFULL(), t & 1);
+      for (int j = 0; j < NJ; ++j) {
+        // FF1(j): h = x W1_j^T
 #pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            float hi[16], lo[16];
-            const float4* bp = reinterpret_cast<const float4*>(g.b1 + j * 128 + cc * 32 + 16 * half);
+        for (int kb = 0; kb < KB; ++kb, ++wb) {
+          const int st = wb % WST;
+          wg::bar_wait(WFULL(st), (wb / WST) & 1);
+          const uint32_t ahi = xbase + (2 * kb) * TILE_B, alo = ahi + TILE_B;
+          const uint32_t bhi = wg::s32(sW + (2 * st) * TILE_B), blo = bhi + TILE_B;
+          wg::pin(h);
+          wg::fence();
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float4 bq = __ldg(bp + q);
-              const float bb[4] = {bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int i = 4 * q + e;
-                const float v = fmaxf(__uint_as_float(rr[16 * half + i]) + bb[e], 0.f);
-                hi[i] = rna(v);
-                lo[i] = v - hi[i];
-              }
-            }
-            tmem_st16(hcol + cc * 32 + 16 * half, hi);
-            tmem_st16(lane_base + COL_HLO + cc * 32 + 16 * half, lo);
+          for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t off = kk * 32;
+            wg::mma_ss_n128(h, wg::desc_sw128(ahi + off, SBO), wg::desc_sw128(bhi + off, SBO), (kb | kk) != 0);
+            wg::mma_ss_n128(h, wg::desc_sw128(alo + off, SBO), wg::desc_sw128(bhi + off, SBO), 1);
+            wg::mma_ss_n128(h, wg::desc_sw128(ahi + off, SBO), wg::desc_sw128(blo + off, SBO), 1);
           }
-        };
-        // this warp group's half of the chunk: columns [64 * eg, 64 * eg + 64)
-        uint32_t r2[32];
-        tmem_ld32_issue(hcol + 64 * eg, r);
-        tmem_ld_wait(r);
-        // H_lo is single-buffered: FF2 of the previous chunk must have retired before it is overwritten
-        if (c >= 1) bar_wait(HFREE(), (c - 1) & 1);
-        tmem_ld32_issue(hcol + 64 * eg + 32, r2);
-        process(r, 2 * eg);
-        tmem_ld_wait(r2);
-        process(r2, 2 * eg + 1);
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        tc_before();
-        bar_arrive(HPFULL());
-      }
-      // final epilogue: Y + b2 + x, BN, store (a lane writes complete 128-byte lines of its own row)
-      bar_wait(YFULL(), t & 1);
-      tc_after();
-      for (int cc = 2 * eg; cc < 2 * eg + 2; ++cc) {
-        tmem_ld32(lane_base + COL_Y + cc * 32, r);
-        if (row < g.M) {
-          const float4* xr = reinterpret_cast<const float4*>(g.x + (size_t)row * g.ldx + cc * 32);
-          float4* dst = reinterpret_cast<float4*>(g.out + (size_t)row * g.ldo + cc * 32);
+          committed(st);
+        }
+        drain();
+        wg::pin(h);
+        if (j == NJ - 1) wg::bar_arrive(XEMPTY());  // the last MMAs that read the x tile have retired
+        // bias + ReLU, H_hi in place; h[4 jj + i]: row m0 + 8 (i / 2), hidden unit 128 j + 8 jj + 2 q + (i % 2)
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 xv = __ldg(xr + q);
-            float y[4] = {__uint_as_float(r[4 * q]) + xv.x, __uint_as_float(r[4 * q + 1]) + xv.y,
-                          __uint_as_float(r[4 * q + 2]) + xv.z, __uint_as_float(r[4 * q + 3]) + xv.w};
-            const float4 bq = __ldg(reinterpret_cast<const float4*>(g.b2 + cc * 32) + q);  // uniform 16-byte loads
-            y[0] += bq.x; y[1] += bq.y; y[2] += bq.z; y[3] += bq.w;
-            if (g.scale) {
-              const float4 sc = __ldg(reinterpret_cast<const float4*>(g.scale + cc * 32) + q);
-              const float4 sh = __ldg(reinterpret_cast<const float4*>(g.shift + cc * 32) + q);
-              y[0] = fmaf(y[0], sc.x, sh.x); y[1] = fmaf(y[1], sc.y, sh.y);
-              y[2] = fmaf(y[2], sc.z, sh.z); y[3] = fmaf(y[3], sc.w, sh.w);
+        for (int jj = 0; jj < 16; ++jj) {
+          const float2 bb = __ldg(reinterpret_cast<const float2*>(g.b1 + j * 128 + 8 * jj + 2 * q));
+          h[4 * jj] = fmaxf(h[4 * jj] + bb.x, 0.f);
+          h[4 * jj + 1] = fmaxf(h[4 * jj + 1] + bb.y, 0.f);
+          h[4 * jj + 2] = fmaxf(h[4 * jj + 2] + bb.x, 0.f);
+          h[4 * jj + 3] = fmaxf(h[4 * jj + 3] + bb.y, 0.f);
+        }
+        // FF2(j): y += h W2_j^T, A from registers (k-step jj = accumulator columns 8 jj .. 8 jj + 7)
+#pragma unroll
+        for (int kb = 0; kb < KB; ++kb, ++wb) {
+          const int st = wb % WST;
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            const int jj = 4 * kb + kk;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {  // A fragment order: (m0, slot q) (m0 + 8, slot q) (m0, q + 4) (m0 + 8, q + 4)
+              float& v = h[4 * jj + ((i & 1) << 1) + (i >> 1)];
+              const float hi = wg::rna_tf32(v);
+              hlo[kb & 1][kk][i] = __float_as_uint(v - hi);
+              v = hi;
             }
-            dst[q] = make_float4(y[0], y[1], y[2], y[3]);
+          }
+          wg::bar_wait(WFULL(st), (wb / WST) & 1);
+          const uint32_t bhi = wg::s32(sW + (2 * st) * TILE_B), blo = bhi + TILE_B;
+          wg::pin(y);
+          wg::fence();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            const int jj = 4 * kb + kk;
+            const uint32_t off = kk * 32;
+            const uint32_t hhi[4] = {__float_as_uint(h[4 * jj]), __float_as_uint(h[4 * jj + 2]), __float_as_uint(h[4 * jj + 1]),
+                                     __float_as_uint(h[4 * jj + 3])};
+            wg::mma_rs_n128(y, hhi, wg::desc_sw128(bhi + off, SBO), (j | kb | kk) != 0);
+            wg::mma_rs_n128(y, hlo[kb & 1][kk], wg::desc_sw128(bhi + off, SBO), 1);
+            wg::mma_rs_n128(y, hhi, wg::desc_sw128(blo + off, SBO), 1);
+          }
+          committed(st);  // leaves this batch in flight; the one that read the other half of hlo has retired
+        }
+        drain();  // FF1(j + 1) overwrites h, the epilogue reads y
+      }
+      wg::pin(y);
+      // final epilogue: Y + b2 + x, BN, store (a quad writes 32 contiguous bytes of a row)
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const int n = 8 * jj + 2 * q;
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(g.b2 + n));
+        float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
+        if (g.scale) { sc = __ldg(reinterpret_cast<const float2*>(g.scale + n)); sh = __ldg(reinterpret_cast<const float2*>(g.shift + n)); }
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int row = m0 + 8 * half;
+          if (row < g.M) {
+            const float2 xv = __ldg(reinterpret_cast<const float2*>(g.x + (size_t)row * g.ldx + n));
+            float2 o = make_float2(y[4 * jj + 2 * half] + xv.x + bb.x, y[4 * jj + 2 * half + 1] + xv.y + bb.y);
+            if (g.scale) { o.x = fmaf(o.x, sc.x, sh.x); o.y = fmaf(o.y, sc.y, sh.y); }
+            *reinterpret_cast<float2*>(g.out + (size_t)row * g.ldo + n) = o;
           }
         }
       }
-      tc_before();
-      bar_arrive(YEMPTY());
     }
   }
-  tc_before();
   __syncthreads();
   cluster_sync();  // no CTA leaves while its peer may still multicast into its shared memory / arrive on its barriers
-  if (warp == 8) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(512));
 }
 
 }  // namespace ffn
@@ -402,11 +279,13 @@ namespace ffn {
 __global__ void __launch_bounds__(256) tile_weights_kernel(const float* __restrict__ w1hi, const float* __restrict__ w1lo,
                                                             const float* __restrict__ w2hi, const float* __restrict__ w2lo,
                                                             float* __restrict__ out) {
-  const int b = blockIdx.x;  // block 0..31
+  const int b = blockIdx.x;  // block 0..WBLOCKS-1
   const WBlock w = wblock(b);
   for (int idx = threadIdx.x; idx < 128 * 32; idx += blockDim.x) {
     const int n = idx >> 5, c = idx & 31;
-    const size_t src = w.ff2 ? (size_t)n * HID + w.j * 128 + w.kb * 32 + c          // W2[n][j*128 + kb*32 + c]
+    // FF2 takes its A operand from the accumulator registers of FF1: k-slot c of W2 holds hidden unit kperm8 (wgmma.cuh)
+    const int k2 = (c & ~7) + wg::kperm8(c & 7);
+    const size_t src = w.ff2 ? (size_t)n * HID + w.j * 128 + w.kb * 32 + k2         // W2[n][j*128 + kb*32 + k2]
                              : ((size_t)w.j * 128 + n) * 128 + w.kb * 32 + c;       // W1[j*128 + n][kb*32 + c]
     const uint32_t off = ((n >> 3) * SBO + (n & 7) * 128 + ((((c >> 2) ^ (n & 7))) << 4) + (c & 3) * 4) >> 2;
     out[(size_t)b * WBLOCK_FLOATS + off] = w.ff2 ? w2hi[src] : w1hi[src];
@@ -416,13 +295,13 @@ __global__ void __launch_bounds__(256) tile_weights_kernel(const float* __restri
 }  // namespace ffn
 }  // namespace co
 
-extern "C" long co_ffn_tiled_weight_floats(void) { return 32L * co::ffn::WBLOCK_FLOATS; }
+extern "C" long co_ffn_tiled_weight_floats(void) { return (long)co::ffn::WBLOCKS * co::ffn::WBLOCK_FLOATS; }
 
 extern "C" int co_ffn_tile_weights(const float* w1hi, const float* w1lo, const float* w2hi, const float* w2lo, float* wtiled,
                                    void* stream) {
   if (!w1hi || !w1lo || !w2hi || !w2lo || !wtiled) return fail(CO_ERR_BAD_ARG, "co_ffn_tile_weights: null pointer%s");
   if ((uintptr_t)wtiled & 127) return fail(CO_ERR_BAD_ARG, "co_ffn_tile_weights: output must be 128-byte aligned%s");
-  co::ffn::tile_weights_kernel<<<32, 256, 0, (cudaStream_t)stream>>>(w1hi, w1lo, w2hi, w2lo, wtiled);
+  co::ffn::tile_weights_kernel<<<co::ffn::WBLOCKS, 256, 0, (cudaStream_t)stream>>>(w1hi, w1lo, w2hi, w2lo, wtiled);
   return check_launch("co_ffn_tile_weights");
 }
 
@@ -443,7 +322,7 @@ extern "C" int co_ffn_fused(const float* x, const float* wtiled, const float* b1
     configured = true;
   }
   const int m_tiles = (M + ffn::BM - 1) / ffn::BM;
-  int grid = device_info().sm_count & ~(ffn::CLUSTER - 1);  // whole clusters (148 = 74 x 2)
+  int grid = device_info().sm_count & ~(ffn::CLUSTER - 1);  // whole clusters
   const int need = (m_tiles + ffn::CLUSTER - 1) & ~(ffn::CLUSTER - 1);
   if (grid > need) grid = need;
   ffn::FfnArgs g{x, wtiled, b1, b2, scale, shift, out, M, ldx, ldo};

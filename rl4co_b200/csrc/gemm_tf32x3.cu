@@ -1,4 +1,4 @@
-// fp32-accurate GEMM on Blackwell tensor cores (tcgen05, kind::tf32, 3xTF32 split).
+// fp32-accurate GEMM on Hopper tensor cores (wgmma, kind tf32, 3xTF32 split).
 //
 //   C[M, Nout] = epilogue( A[M, K] @ W[Nout, K]^T )        A, W, C: fp32 row-major
 //   epilogue(v) = ((v + bias[n]) (+ residual[m, n])) (relu) * scale[n] + shift[n]
@@ -11,68 +11,41 @@
 //     into the epilogue.
 //
 // Numerics: each fp32 operand x is split into hi = rna_tf32(x) and lo = x - hi; the kernel
-// accumulates hi*hi + lo*hi + hi*lo in fp32 TMEM accumulators (the dropped lo*lo term is
+// accumulates hi*hi + lo*hi + hi*lo in fp32 register accumulators (the dropped lo*lo term is
 // ~2^-22 relative), i.e. fp32-class accuracy (~1e-6 relative) at tensor-core rate.
 //
-// Structure (one CTA per 128x128 output tile, 256 threads, 64 KB smem, 2-3 CTAs/SM overlap each
-// other's load / MMA / epilogue phases):
-//   per 32-wide k-block: the k-block's A / W_hi / W_lo float4s are prefetched into registers
-//   while the previous k-block's MMAs run; then split A -> STS into 128-byte-swizzled K-major
-//   tiles (row r at r*128 B, 16-byte chunk c stored at c ^ (r & 7); SBO = 1 KB) ->
-//   fence.proxy.async -> one elected thread issues 12 tcgen05.mma.kind::tf32 (4 k-steps x 3
-//   products hi*hi, lo*hi, hi*lo) -> tcgen05.commit -> mbarrier.
-//   Epilogue: all 8 warps tcgen05.ld 32x32b.x32 their TMEM lanes, transpose through swizzled
-//   shared memory, apply the fused epilogue and store full 128-byte row segments.
-#include <stdlib.h>
-
+// Structure: persistent CTAs of three warpgroups; a CTA keeps one 128-column block of W and walks over 128-row tiles.
+//   warpgroup 0  producer : LDG the next 32-wide k-block of A (one block ahead, in registers) -> hi / lo split -> STS
+//                           into a 3-stage ring of 128-byte-swizzled K-major tiles (row r at r*128 B, 16-byte chunk c
+//                           stored at c ^ (r & 7); SBO = 1 KB) -> fence.proxy.async -> mbarrier "full"
+//   warpgroups 1-2 consumers: 64 rows x 128 columns each; per k-block 12 wgmma m64n128k8 (4 k-steps x 3 products
+//                           hi*hi, lo*hi, hi*lo), one batch in flight while the previous stage is released; the fused
+//                           epilogue runs from the accumulator registers (a quad stores 32 contiguous bytes of a row)
+//                           while the producer already fills the ring for the next tile.
+//   K == 128 (every projection of the encoder / cache): the CTA's W block (hi + lo, 128 KB) stays in shared memory and
+//   the ring carries A only; otherwise the ring stages carry the k-block of W as well.
 #include "co_common.cuh"
+#include "wgmma.cuh"
 
 namespace co {
 
 constexpr int GM = 128, GN = 128, GK = 32;
 constexpr int TILE_BYTES = GM * GK * 4;  // 16 KB per operand tile
-constexpr uint32_t SBO = 1024;  // 8 rows x 128 B swizzle atom
+constexpr uint32_t SBO = 1024;           // 8 rows x 128 B swizzle atom
+constexpr int KB128 = 4;                 // k-blocks of the W-stationary variant
+constexpr int STAGES = 3;
+constexpr int GEMM_THREADS = 384;
+constexpr int GEMM_SMEM = 2 * KB128 * TILE_BYTES + STAGES * 2 * TILE_BYTES;  // == STAGES * 4 * TILE_BYTES + 32 KB spare
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  // cute::UMMA::SmemDescriptor (mma_sm100_desc.hpp): start>>4 [0,14), LBO>>4 [16,30) (unused
-  // for swizzled K-major, canonical value 1), SBO>>4 [32,46), version=1 [46,48),
-  // layout_type=SWIZZLE_128B (2) [61,64)
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(SBO >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// cute::UMMA::InstrDescriptor: c_format=F32 (1<<4), a/b_format=TF32 (2<<7, 2<<10), K-major both,
-// n_dim = N>>3 at [17,23), m_dim = M>>4 at [24,29)
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((GN >> 3) << 17) | ((GM >> 4) << 24);
-
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ float rna_tf32(float v) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-  return __uint_as_float(u);
-}
 __device__ __forceinline__ float4 split_hi(float4 v) {
-  return make_float4(rna_tf32(v.x), rna_tf32(v.y), rna_tf32(v.z), rna_tf32(v.w));
+  return make_float4(wg::rna_tf32(v.x), wg::rna_tf32(v.y), wg::rna_tf32(v.z), wg::rna_tf32(v.w));
 }
+__device__ __forceinline__ float4 sub4(float4 a, float4 b) { return make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w); }
 
 __global__ void split_tf32_kernel(const float* __restrict__ w, float* __restrict__ hi, float* __restrict__ lo, long n) {
   long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
-    const float v = w[i], h = rna_tf32(v);
+    const float v = w[i], h = wg::rna_tf32(v);
     hi[i] = h;
     lo[i] = v - h;
   }
@@ -84,339 +57,68 @@ struct GemmArgs {
   int M, Nout, K, lda, ldc, ldr, relu, n_tiles;
 };
 
-// all 8 warps: warp w reads TMEM lanes 32(w%4).. (rows) x 64 columns [(w/4)*64, +64), transposes
-// through chunk-swizzled shared memory (`smem`: 8 x 4 KB) and stores 4 rows x 128 B per instruction
-__device__ __forceinline__ void epilogue_chunks(const GemmArgs& g, float* stage, uint32_t tmem_d, int m0, int n0, int wq,
-                                                int cc_begin, int cc_count, int lane);
-__device__ __forceinline__ void epilogue_tile(const GemmArgs& g, unsigned char* smem, uint32_t tmem_d, int m0, int n0,
-                                              int warp, int lane) {
-  epilogue_chunks(g, reinterpret_cast<float*>(smem) + warp * 1024, tmem_d, m0, n0, warp & 3, (warp >> 2) * 2, 2, lane);
-}
-// warp-level: rows 32*wq.. of the tile, column chunks [cc_begin, cc_begin + cc_count) of 32 columns each
-__device__ __forceinline__ void epilogue_chunks(const GemmArgs& g, float* stage, uint32_t tmem_d, int m0, int n0, int wq,
-                                                int cc_begin, int cc_count, int lane) {
-  {
-    const int rr = lane >> 3, v = lane & 7;  // store mapping: 4 rows x 8 chunks per instruction
-#pragma unroll 1
-    for (int c2 = 0; c2 < cc_count; ++c2) {
-      const int cc = cc_begin + c2;
-      // operands of the fused epilogue first: their latency hides behind the TMEM read + transpose
-      const int n = n0 + cc * 32 + 4 * v;
-      const bool n_ok = n < g.Nout;
-      float4 bs = make_float4(0.f, 0.f, 0.f, 0.f), sc4 = make_float4(1.f, 1.f, 1.f, 1.f), sh4 = bs;
-      if (n_ok && g.bias) bs = __ldg(reinterpret_cast<const float4*>(g.bias + n));
-      if (n_ok && g.scale) { sc4 = __ldg(reinterpret_cast<const float4*>(g.scale + n)); sh4 = __ldg(reinterpret_cast<const float4*>(g.shift + n)); }
-      float4 res[8];
+// fused epilogue of one consumer warpgroup straight from its accumulator fragment: rows m0 + {g, g + 8}, column pairs
+// n0 + 8 j + 2 q (wgmma.cuh)
+__device__ __forceinline__ void epilogue_regs(const GemmArgs& g, const float (&d)[64], int m0, int n0, int lane) {
+  const int q = lane & 3;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int n = n0 + 8 * j + 2 * q;
+    if (n >= g.Nout) continue;
+    float2 bs = make_float2(0.f, 0.f), sc = make_float2(1.f, 1.f), sh = bs;
+    if (g.bias) bs = __ldg(reinterpret_cast<const float2*>(g.bias + n));
+    if (g.scale) { sc = __ldg(reinterpret_cast<const float2*>(g.scale + n)); sh = __ldg(reinterpret_cast<const float2*>(g.shift + n)); }
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int row = m0 + (lane >> 2) + 8 * half;
+      if (row >= g.M) continue;
+      float2 o = make_float2(d[4 * j + 2 * half] + bs.x, d[4 * j + 2 * half + 1] + bs.y);
       if (g.residual) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int row = m0 + 32 * wq + 4 * i + rr;
-          res[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          // plain (coherent) load: the residual may alias C (in-place accumulation across split-K passes)
-          if (row < g.M && n_ok) res[i] = *reinterpret_cast<const float4*>(g.residual + (size_t)row * g.ldr + n);
-        }
+        // plain (coherent) load: the residual may alias C (in-place accumulation across split-K passes)
+        const float2 r = *reinterpret_cast<const float2*>(g.residual + (size_t)row * g.ldr + n);
+        o.x += r.x; o.y += r.y;
       }
-      uint32_t r[32];
-      const uint32_t taddr = tmem_d + ((uint32_t)(32 * wq) << 16) + cc * 32;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-            "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-            "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-            "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int u = 0; u < 8; ++u)  // thread = row `lane`: chunk u stored at u ^ (lane & 7)
-        *reinterpret_cast<uint4*>(stage + lane * 32 + ((u ^ (lane & 7)) << 2)) = make_uint4(r[4 * u], r[4 * u + 1], r[4 * u + 2], r[4 * u + 3]);
-      __syncwarp();
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int lrow = 4 * i + rr;
-        const int row = m0 + 32 * wq + lrow;
-        float4 o = *reinterpret_cast<const float4*>(stage + lrow * 32 + ((v ^ (lrow & 7)) << 2));
-        if (row < g.M && n_ok) {
-          o.x += bs.x; o.y += bs.y; o.z += bs.z; o.w += bs.w;
-          if (g.residual) { o.x += res[i].x; o.y += res[i].y; o.z += res[i].z; o.w += res[i].w; }
-          if (g.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-          if (g.scale) { o.x = fmaf(o.x, sc4.x, sh4.x); o.y = fmaf(o.y, sc4.y, sh4.y); o.z = fmaf(o.z, sc4.z, sh4.z); o.w = fmaf(o.w, sc4.w, sh4.w); }
-          *reinterpret_cast<float4*>(g.C + (size_t)row * g.ldc + n) = o;
-        }
-      }
-      __syncwarp();
+      if (g.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+      if (g.scale) { o.x = fmaf(o.x, sc.x, sh.x); o.y = fmaf(o.y, sc.y, sh.y); }
+      *reinterpret_cast<float2*>(g.C + (size_t)row * g.ldc + n) = o;
     }
   }
 }
 
-__global__ void __launch_bounds__(256, 2) gemm_tf32x3_kernel(const GemmArgs g) {
+// one k-block of a producer thread: 8 x (4 rows x 128 B) of A and, unless W is resident, of W_hi / W_lo
+template <bool WSTAT>
+struct KBlock {
+  float4 a[8];
+  float4 h[WSTAT ? 1 : 8], l[WSTAT ? 1 : 8];
+};
+
+template <bool WSTAT>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tf32x3_kernel(const GemmArgs g, int m_tiles, int groups) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  unsigned char* sAhi = smem;
-  unsigned char* sAlo = smem + TILE_BYTES;
-  unsigned char* sBhi = smem + 2 * TILE_BYTES;
-  unsigned char* sBlo = smem + 3 * TILE_BYTES;
-  __shared__ __align__(8) uint64_t mbar;
-  __shared__ uint32_t tmem_base_s;
+  // WSTAT: [kb][W_hi, W_lo] (128 KB) then the ring of [A_hi, A_lo]; else a ring of [A_hi, A_lo, W_hi, W_lo]
+  constexpr int STAGE_BYTES = (WSTAT ? 2 : 4) * TILE_BYTES;
+  unsigned char* sW = smem;
+  unsigned char* sRing = smem + (WSTAT ? 2 * KB128 * TILE_BYTES : 0);
+  __shared__ __align__(8) uint64_t bars[2 * STAGES];  // full[STAGES] (128 producers), empty[STAGES] (256 consumers)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n_tile = blockIdx.x % g.n_tiles, m_tile = blockIdx.x / g.n_tiles;  // N fastest: A tile reused from L2
-  const int m0 = m_tile * GM, n0 = n_tile * GN;
-
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(GN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 32) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&mbar)));
-    asm volatile("fence.mbarrier_init.release.cluster;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;");
-  const uint32_t tmem_d = tmem_base_s;
-
-  // load mapping: a warp covers 8 rows x 4 chunks(16 B): 8 x 64 B global segments, and -- with the
-  // 128B swizzle -- 8 distinct bank groups per quarter-warp on the shared-memory side
-  const int r8 = lane & 7, c4 = lane >> 3;
+  const int n_tile = blockIdx.x % g.n_tiles, group = blockIdx.x / g.n_tiles;
+  const int n0 = n_tile * GN;
   const int nkb = g.K / GK;
-  float4 pa[4], ph[4], pl[4];
-  auto prefetch = [&](int kb) {
-    const int k0 = kb * GK;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int q = warp + 8 * j;  // 32 (row-group, chunk-half) items per tile
-      const int row = 8 * (q >> 1) + r8, chunk = 4 * (q & 1) + c4;
-      pa[j] = make_float4(0.f, 0.f, 0.f, 0.f); ph[j] = pa[j]; pl[j] = pa[j];
-      if (m0 + row < g.M) pa[j] = __ldg(reinterpret_cast<const float4*>(g.A + (size_t)(m0 + row) * g.lda + k0 + chunk * 4));
-      if (n0 + row < g.Nout) {
-        ph[j] = __ldg(reinterpret_cast<const float4*>(g.Whi + (size_t)(n0 + row) * g.K + k0 + chunk * 4));
-        pl[j] = __ldg(reinterpret_cast<const float4*>(g.Wlo + (size_t)(n0 + row) * g.K + k0 + chunk * 4));
-      }
-    }
-  };
-  auto wait_mma = [&](uint32_t parity) {
-    uint32_t done = 0;
-    const uint32_t bar = smem_u32(&mbar);
-    while (!done) {
-      asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}"
-                   : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    }
-  };
-  prefetch(0);
-  for (int kb = 0; kb < nkb; ++kb) {
-    if (kb > 0) wait_mma((kb - 1) & 1);  // MMAs of the previous k-block have consumed the smem stage
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int q = warp + 8 * j;
-      const int rg = q >> 1, chunk = 4 * (q & 1) + c4;
-      const uint32_t soff = rg * SBO + r8 * 128 + ((chunk ^ r8) << 4);
-      const float4 ah = split_hi(pa[j]);
-      const float4 al = make_float4(pa[j].x - ah.x, pa[j].y - ah.y, pa[j].z - ah.z, pa[j].w - ah.w);
-      *reinterpret_cast<float4*>(sAhi + soff) = ah;
-      *reinterpret_cast<float4*>(sAlo + soff) = al;
-      *reinterpret_cast<float4*>(sBhi + soff) = ph[j];
-      *reinterpret_cast<float4*>(sBlo + soff) = pl[j];
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> async-proxy (MMA) reads
-    __syncthreads();
-    if (kb + 1 < nkb) prefetch(kb + 1);  // global loads fly while the tensor core works
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;");
-      const uint32_t ahi = smem_u32(sAhi), alo = smem_u32(sAlo), bhi = smem_u32(sBhi), blo = smem_u32(sBlo);
-#pragma unroll
-      for (int kk = 0; kk < GK / 8; ++kk) {  // UMMA_K = 8 tf32 = 32 B: advance inside the swizzle atom
-        const uint32_t off = kk * 32;
-        mma_tf32(tmem_d, make_desc(ahi + off), make_desc(bhi + off), (kb | kk) != 0);
-        mma_tf32(tmem_d, make_desc(alo + off), make_desc(bhi + off), 1);
-        mma_tf32(tmem_d, make_desc(ahi + off), make_desc(blo + off), 1);
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&mbar)) : "memory");
-    }
-  }
-  wait_mma((nkb - 1) & 1);  // accumulator complete; operand tiles free (reused as staging below)
-  asm volatile("tcgen05.fence::after_thread_sync;");
-
-  epilogue_tile(g, smem, tmem_d, m0, n0, warp, lane);
-  asm volatile("tcgen05.fence::before_thread_sync;");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(GN));
-  }
-}
-
-
-// ---- W-stationary variant for K == 128 (all the K=128 projections of the path): a persistent CTA
-// keeps its 128-column W tile (hi + lo, 4 k-blocks, 128 KB) in shared memory and streams M tiles
-// through one 32 KB A stage, so per output tile only the 64 KB A tile crosses L2 -> SM.
-constexpr int KB128 = 4;
-__global__ void __launch_bounds__(256, 1) gemm_tf32x3_wstat_kernel(const GemmArgs g, int m_tiles, int groups) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  unsigned char* sAhi = smem;                    // also the epilogue staging (8 x 4 KB)
-  unsigned char* sAlo = smem + TILE_BYTES;
-  unsigned char* sW = smem + 2 * TILE_BYTES;     // [kb][hi, lo] 16 KB each
-  __shared__ __align__(8) uint64_t mbar;
-  __shared__ uint32_t tmem_base_s;
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n_tile = blockIdx.x % g.n_tiles, group = blockIdx.x / g.n_tiles;
-  const int n0 = n_tile * GN;
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(GN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 32) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&mbar)));
-    asm volatile("fence.mbarrier_init.release.cluster;");
-  }
-  const int r8 = lane & 7, c4 = lane >> 3;
-  // resident W tile
-  for (int kb = 0; kb < KB128; ++kb) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int q = warp + 8 * j;
-      const int rg = q >> 1, chunk = 4 * (q & 1) + c4, row = 8 * rg + r8;
-      const uint32_t soff = rg * SBO + r8 * 128 + ((chunk ^ r8) << 4);
-      float4 h = make_float4(0.f, 0.f, 0.f, 0.f), l = h;
-      if (n0 + row < g.Nout) {
-        h = __ldg(reinterpret_cast<const float4*>(g.Whi + (size_t)(n0 + row) * g.K + kb * GK + chunk * 4));
-        l = __ldg(reinterpret_cast<const float4*>(g.Wlo + (size_t)(n0 + row) * g.K + kb * GK + chunk * 4));
-      }
-      *reinterpret_cast<float4*>(sW + (2 * kb) * TILE_BYTES + soff) = h;
-      *reinterpret_cast<float4*>(sW + (2 * kb + 1) * TILE_BYTES + soff) = l;
-    }
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;");
-  const uint32_t tmem_d = tmem_base_s;
-
-  float4 pa[4];
-  auto prefetch = [&](int mt, int kb) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int q = warp + 8 * j;
-      const int row = mt * GM + 8 * (q >> 1) + r8, chunk = 4 * (q & 1) + c4;
-      pa[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (mt < m_tiles && row < g.M) pa[j] = __ldg(reinterpret_cast<const float4*>(g.A + (size_t)row * g.lda + kb * GK + chunk * 4));
-    }
-  };
-  uint32_t commits = 0;  // number of tcgen05.commit issued so far (mbarrier phase = commits & 1)
-  auto wait_mma = [&](uint32_t parity) {
-    uint32_t done = 0;
-    const uint32_t bar = smem_u32(&mbar);
-    while (!done) {
-      asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}"
-                   : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    }
-  };
-  int mt = group;
-  prefetch(mt, 0);
-  for (; mt < m_tiles; mt += groups) {
-    for (int kb = 0; kb < KB128; ++kb) {
-      if (kb > 0) wait_mma((commits - 1) & 1);  // previous k-block's MMAs have consumed the A stage
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int q = warp + 8 * j;
-        const int rg = q >> 1, chunk = 4 * (q & 1) + c4;
-        const uint32_t soff = rg * SBO + r8 * 128 + ((chunk ^ r8) << 4);
-        const float4 ah = split_hi(pa[j]);
-        *reinterpret_cast<float4*>(sAhi + soff) = ah;
-        *reinterpret_cast<float4*>(sAlo + soff) = make_float4(pa[j].x - ah.x, pa[j].y - ah.y, pa[j].z - ah.z, pa[j].w - ah.w);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncthreads();
-      if (kb + 1 < KB128) prefetch(mt, kb + 1); else prefetch(mt + groups, 0);
-      if (tid == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;");
-        const uint32_t ahi = smem_u32(sAhi), alo = smem_u32(sAlo);
-        const uint32_t bhi = smem_u32(sW + (2 * kb) * TILE_BYTES), blo = smem_u32(sW + (2 * kb + 1) * TILE_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < GK / 8; ++kk) {
-          const uint32_t off = kk * 32;
-          mma_tf32(tmem_d, make_desc(ahi + off), make_desc(bhi + off), (kb | kk) != 0);
-          mma_tf32(tmem_d, make_desc(alo + off), make_desc(bhi + off), 1);
-          mma_tf32(tmem_d, make_desc(ahi + off), make_desc(blo + off), 1);
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&mbar)) : "memory");
-      }
-      ++commits;
-    }
-    wait_mma((commits - 1) & 1);  // accumulator complete, A stage free (reused as staging)
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    epilogue_tile(g, smem, tmem_d, mt * GM, n0, warp, lane);
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();  // staging reads and TMEM reads done before the next tile's stores / MMAs
-    asm volatile("tcgen05.fence::after_thread_sync;");
-  }
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(GN));
-}
-
-
-// ---- warp-specialised W-stationary pipeline for K == 128 (the fast path):
-//   warps 0-3  producers : LDG A (one full tile = 4 k-blocks prefetched in registers a tile ahead)
-//                          -> hi/lo split -> STS into a 2-stage ring of swizzled A tiles
-//   warps 4-7  epilogue  : TMEM -> registers -> swizzled staging -> fused epilogue -> 128 B row stores
-//   warp  8    MMA issuer: waits full[s], issues 12 tcgen05.mma per k-block, commits to empty[s];
-//                          accumulators double-buffered in TMEM (2 x 128 columns)
-// so loads, tensor-core work and stores of consecutive tiles overlap inside one persistent CTA.
-constexpr int PIPE_THREADS = 288;
-constexpr int A_STAGES = 2;
-constexpr int PIPE_SMEM = 2 * KB128 * TILE_BYTES + A_STAGES * 2 * TILE_BYTES + 4 * 4096;
-
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  }
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-__global__ void __launch_bounds__(PIPE_THREADS, 1) gemm_tf32x3_pipe_kernel(const GemmArgs g, int m_tiles, int groups) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  unsigned char* sW = smem;                                   // [kb][hi, lo] 16 KB each (128 KB)
-  unsigned char* sA = smem + 2 * KB128 * TILE_BYTES;          // [stage][hi, lo]
-  float* sStage = reinterpret_cast<float*>(sA + A_STAGES * 2 * TILE_BYTES);  // 4 x 4 KB
-  __shared__ __align__(8) uint64_t bars[2 * A_STAGES + 4];    // full[2], empty[2], tfull[2], tempty[2]
-  __shared__ uint32_t tmem_base_s;
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n_tile = blockIdx.x % g.n_tiles, group = blockIdx.x / g.n_tiles;
-  const int n0 = n_tile * GN;
-  const uint32_t bar0 = smem_u32(bars);
+  const uint32_t bar0 = wg::s32(bars);
   auto FULL_B = [&](int s) { return bar0 + 8 * s; };
-  auto EMPTY_B = [&](int s) { return bar0 + 8 * (A_STAGES + s); };
-  auto TFULL_B = [&](int a) { return bar0 + 8 * (2 * A_STAGES + a); };
-  auto TEMPTY_B = [&](int a) { return bar0 + 8 * (2 * A_STAGES + 2 + a); };
+  auto EMPTY_B = [&](int s) { return bar0 + 8 * (STAGES + s); };
 
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(2 * GN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
-    for (int s = 0; s < A_STAGES; ++s) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(FULL_B(s)), "r"(128));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(EMPTY_B(s)), "r"(1));
-    }
-    for (int a = 0; a < 2; ++a) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(TFULL_B(a)), "r"(1));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(TEMPTY_B(a)), "r"(128));
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;");
+    for (int s = 0; s < STAGES; ++s) { wg::bar_init(FULL_B(s), 128); wg::bar_init(EMPTY_B(s), 256); }
+    wg::bar_init_fence();
   }
-  // resident W tile: all 288 threads, item = (kb, row-group, chunk-half); a warp covers 8 rows x 4 chunks
-  {
+  if (WSTAT) {
+    // resident W block: item = (kb, row-group, chunk-half); a warp covers 8 rows x 4 chunks
     const int r8 = lane & 7, c4 = lane >> 3;
-    for (int item = warp; item < KB128 * 32; item += PIPE_THREADS / 32) {
-      const int kb = item >> 5, q = item & 31;
-      const int rg = q >> 1, chunk = 4 * (q & 1) + c4, row = 8 * rg + r8;
+    for (int item = warp; item < KB128 * 32; item += GEMM_THREADS / 32) {
+      const int kb = item >> 5, qq = item & 31;
+      const int rg = qq >> 1, chunk = 4 * (qq & 1) + c4, row = 8 * rg + r8;
       const uint32_t soff = rg * SBO + r8 * 128 + ((chunk ^ r8) << 4);
       float4 h = make_float4(0.f, 0.f, 0.f, 0.f), l = h;
       if (n0 + row < g.Nout) {
@@ -426,96 +128,93 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) gemm_tf32x3_pipe_kernel(const
       *reinterpret_cast<float4*>(sW + (2 * kb) * TILE_BYTES + soff) = h;
       *reinterpret_cast<float4*>(sW + (2 * kb + 1) * TILE_BYTES + soff) = l;
     }
+    wg::fence_async();
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;");
-  const uint32_t tmem_d = tmem_base_s;
 
   if (warp < 4) {
-    // ------------------------------------------------------------------ producers
+    // ------------------------------------------------------------------ producer warpgroup
     // lane -> (row % 4, 16-byte chunk 0..7): every LDG.128 instruction fetches 4 complete 128-byte
     // rows of the k-block, and a quarter-warp writes one swizzled 128-byte row (conflict-free)
     const int r4 = lane >> 3, c8 = lane & 7;
-    float4 R[KB128][8];
-    auto prefetch = [&](int mt, int kb) {
+    auto load = [&](int mt, int kb, auto& R) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const int row = mt * GM + 16 * j + 4 * warp + r4;
-        R[kb][j] = make_float4(0.f, 0.f, 0.f, 0.f);
+        const int lrow = 16 * j + 4 * warp + r4;
+        const int row = mt * GM + lrow;
+        R.a[j] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (mt < m_tiles && row < g.M)
-          R[kb][j] = __ldg(reinterpret_cast<const float4*>(g.A + (size_t)row * g.lda + kb * GK + c8 * 4));
+          R.a[j] = __ldg(reinterpret_cast<const float4*>(g.A + (size_t)row * g.lda + kb * GK + c8 * 4));
+        if constexpr (!WSTAT) {
+          R.h[j] = R.l[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (mt < m_tiles && n0 + lrow < g.Nout) {
+            R.h[j] = __ldg(reinterpret_cast<const float4*>(g.Whi + (size_t)(n0 + lrow) * g.K + kb * GK + c8 * 4));
+            R.l[j] = __ldg(reinterpret_cast<const float4*>(g.Wlo + (size_t)(n0 + lrow) * g.K + kb * GK + c8 * 4));
+          }
+        }
       }
     };
-#pragma unroll
-    for (int kb = 0; kb < KB128; ++kb) prefetch(group, kb);
+    KBlock<WSTAT> R;
+    KBlock<true> Rn;  // W-stationary: a second register set keeps the next block of A in flight
+    load(group, 0, R);
     uint32_t it = 0;
     for (int mt = group; mt < m_tiles; mt += groups) {
-#pragma unroll
-      for (int kb = 0; kb < KB128; ++kb) {
-        const int s = it & 1;
-        mbar_wait(EMPTY_B(s), ((it >> 1) & 1) ^ 1);
-        unsigned char* ahi = sA + (2 * s) * TILE_BYTES;
-        unsigned char* alo = ahi + TILE_BYTES;
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        auto load_next = [&](auto& dst) { if (kb + 1 < nkb) load(mt, kb + 1, dst); else load(mt + groups, 0, dst); };
+        if constexpr (WSTAT) load_next(Rn);
+        const int s = it % STAGES;
+        wg::bar_wait(EMPTY_B(s), ((it / STAGES) & 1) ^ 1);
+        unsigned char* st = sRing + s * STAGE_BYTES;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int lrow = 16 * j + 4 * warp + r4;  // row within the tile
           const uint32_t soff = (lrow >> 3) * SBO + (lrow & 7) * 128 + ((c8 ^ (lrow & 7)) << 4);
-          const float4 a = R[kb][j], h = split_hi(a);
-          *reinterpret_cast<float4*>(ahi + soff) = h;
-          *reinterpret_cast<float4*>(alo + soff) = make_float4(a.x - h.x, a.y - h.y, a.z - h.z, a.w - h.w);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_arrive(FULL_B(s));
-        prefetch(mt + groups, kb);  // same k-block of the next tile: a whole tile time to land
-        ++it;
-      }
-    }
-  } else if (warp == 8) {
-    // ------------------------------------------------------------------ MMA issuer (one thread)
-    if (lane == 0) {
-      uint32_t it = 0, tc = 0;
-      for (int mt = group; mt < m_tiles; mt += groups, ++tc) {
-        const int acc = tc & 1;
-        mbar_wait(TEMPTY_B(acc), ((tc >> 1) & 1) ^ 1);
-        asm volatile("tcgen05.fence::after_thread_sync;");
-        const uint32_t d = tmem_d + acc * GN;
-        for (int kb = 0; kb < KB128; ++kb, ++it) {
-          const int s = it & 1;
-          mbar_wait(FULL_B(s), (it >> 1) & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;");
-          const uint32_t ahi = smem_u32(sA + (2 * s) * TILE_BYTES), alo = ahi + TILE_BYTES;
-          const uint32_t bhi = smem_u32(sW + (2 * kb) * TILE_BYTES), blo = bhi + TILE_BYTES;
-#pragma unroll
-          for (int kk = 0; kk < GK / 8; ++kk) {
-            const uint32_t off = kk * 32;
-            mma_tf32(d, make_desc(ahi + off), make_desc(bhi + off), (kb | kk) != 0);
-            mma_tf32(d, make_desc(alo + off), make_desc(bhi + off), 1);
-            mma_tf32(d, make_desc(ahi + off), make_desc(blo + off), 1);
+          const float4 h = split_hi(R.a[j]);
+          *reinterpret_cast<float4*>(st + soff) = h;
+          *reinterpret_cast<float4*>(st + TILE_BYTES + soff) = sub4(R.a[j], h);
+          if (!WSTAT) {
+            *reinterpret_cast<float4*>(st + 2 * TILE_BYTES + soff) = R.h[j];
+            *reinterpret_cast<float4*>(st + 3 * TILE_BYTES + soff) = R.l[j];
           }
-          umma_commit(EMPTY_B(s));  // A stage reusable once these MMAs have read it
         }
-        umma_commit(TFULL_B(acc));  // accumulator complete
+        wg::fence_async();  // generic-proxy stores -> async-proxy (MMA) reads
+        wg::bar_arrive(FULL_B(s));
+        if constexpr (WSTAT) R = Rn; else load_next(R);
       }
     }
-    __syncwarp();
   } else {
-    // ------------------------------------------------------------------ epilogue warps 4..7
-    const int wq = warp & 3;
-    uint32_t tc = 0;
-    for (int mt = group; mt < m_tiles; mt += groups, ++tc) {
-      const int acc = tc & 1;
-      mbar_wait(TFULL_B(acc), (tc >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;");
-      epilogue_chunks(g, sStage + wq * 1024, tmem_d + acc * GN, mt * GM, n0, wq, 0, GN / 32, lane);
-      asm volatile("tcgen05.fence::before_thread_sync;");
-      mbar_arrive(TEMPTY_B(acc));
+    // ------------------------------------------------------------------ consumer warpgroups: 64 rows each
+    const int cw = (warp - 4) >> 2, w4 = warp & 3;
+    uint32_t it = 0;
+    float d[64];
+    for (int mt = group; mt < m_tiles; mt += groups) {
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const int s = it % STAGES;
+        wg::bar_wait(FULL_B(s), (it / STAGES) & 1);
+        const uint32_t ahi = wg::s32(sRing + s * STAGE_BYTES) + cw * 64 * 128, alo = ahi + TILE_BYTES;
+        const uint32_t bhi = WSTAT ? wg::s32(sW + (2 * kb) * TILE_BYTES) : wg::s32(sRing + s * STAGE_BYTES + 2 * TILE_BYTES);
+        const uint32_t blo = bhi + TILE_BYTES;
+        wg::pin(d);
+        wg::fence();
+#pragma unroll
+        for (int kk = 0; kk < GK / 8; ++kk) {  // one k-step = 8 tf32 = 32 B: advance inside the swizzle atom
+          const uint32_t off = kk * 32;
+          wg::mma_ss_n128(d, wg::desc_sw128(ahi + off, SBO), wg::desc_sw128(bhi + off, SBO), (kb | kk) != 0);
+          wg::mma_ss_n128(d, wg::desc_sw128(alo + off, SBO), wg::desc_sw128(bhi + off, SBO), 1);
+          wg::mma_ss_n128(d, wg::desc_sw128(ahi + off, SBO), wg::desc_sw128(blo + off, SBO), 1);
+        }
+        wg::commit();
+        if (kb > 0) {  // the previous k-block's MMAs have retired: its stage goes back to the producer
+          wg::wait<1>();
+          wg::bar_arrive(EMPTY_B((it - 1) % STAGES));
+        }
+      }
+      wg::wait<0>();
+      wg::pin(d);
+      wg::bar_arrive(EMPTY_B((it - 1) % STAGES));
+      epilogue_regs(g, d, mt * GM + 64 * cw + 16 * w4, n0, lane);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;");
-  __syncthreads();
-  if (warp == 8) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(2 * GN));
 }
 
 }  // namespace co
@@ -542,31 +241,24 @@ extern "C" int co_gemm_tf32x3(const float* A, const float* Whi, const float* Wlo
     return fail(CO_ERR_BAD_ARG, "co_gemm_tf32x3: pointers must be 16-byte aligned%s");
   if (M == 0) return CO_OK;
   GemmArgs g{A, Whi, Wlo, C, bias, residual, scale, shift, M, Nout, K, lda, ldc, ldr, relu, (Nout + GN - 1) / GN};
-  const long tiles = (long)((M + GM - 1) / GM) * g.n_tiles;
-  if (tiles > 0x7fffffffL) return fail(CO_ERR_UNSUPPORTED, "co_gemm_tf32x3: too many tiles%s");
+  const int m_tiles = (M + GM - 1) / GM;
+  if ((long)m_tiles * g.n_tiles > 0x7fffffffL) return fail(CO_ERR_UNSUPPORTED, "co_gemm_tf32x3: too many tiles%s");
   static PerDeviceOnce once;
   bool& configured = once.flag();
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * TILE_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gemm_tf32x3_wstat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (2 + 2 * KB128) * TILE_BYTES);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gemm_tf32x3_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PIPE_SMEM);
+      e = cudaFuncSetAttribute(gemm_tf32x3_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGES * 4 * TILE_BYTES);
     if (e != cudaSuccess) return fail(CO_ERR_CUDA, "co_gemm_tf32x3: smem attribute: %s", cudaGetErrorString(e));
     configured = true;
   }
-  const int m_tiles = (M + GM - 1) / GM;
-  const int sms = device_info().sm_count;
-  if (K == GK * KB128 && g.n_tiles <= sms && m_tiles >= 4 * (sms / g.n_tiles)) {
-    const int groups = sms / g.n_tiles;  // CTAs of one group share an M tile (L2 reuse of A)
-    static const int variant = getenv("CO_GEMM_VARIANT") ? atoi(getenv("CO_GEMM_VARIANT")) : 2;
-    if (variant == 1) {
-      gemm_tf32x3_wstat_kernel<<<groups * g.n_tiles, 256, (2 + 2 * KB128) * TILE_BYTES, (cudaStream_t)stream>>>(g, m_tiles, groups);
-      return check_launch("co_gemm_tf32x3(wstat)");
-    }
-    gemm_tf32x3_pipe_kernel<<<groups * g.n_tiles, PIPE_THREADS, PIPE_SMEM, (cudaStream_t)stream>>>(g, m_tiles, groups);
-    return check_launch("co_gemm_tf32x3(pipe)");
-  }
-  gemm_tf32x3_kernel<<<(unsigned)tiles, 256, 4 * TILE_BYTES, (cudaStream_t)stream>>>(g);
+  // CTAs of one group share an M tile (L2 reuse of A); every CTA keeps its block of W columns
+  int groups = device_info().sm_count / g.n_tiles;
+  if (groups < 1) groups = 1;
+  if (groups > m_tiles) groups = m_tiles;
+  if (K == GK * KB128)
+    gemm_tf32x3_kernel<true><<<groups * g.n_tiles, GEMM_THREADS, GEMM_SMEM, (cudaStream_t)stream>>>(g, m_tiles, groups);
+  else
+    gemm_tf32x3_kernel<false><<<groups * g.n_tiles, GEMM_THREADS, STAGES * 4 * TILE_BYTES, (cudaStream_t)stream>>>(g, m_tiles, groups);
   return check_launch("co_gemm_tf32x3");
 }

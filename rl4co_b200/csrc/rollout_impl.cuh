@@ -10,15 +10,14 @@
 //   TSPEnv._step / CVRPEnv._step       envs/routing/tsp/env.py:60-86, cvrp/env.py:66-136
 // and at the end get_reward (ops.py:82-90) and get_log_likelihood (decoding.py:38-62).
 //
-// Design (B200, fourth version -- the per-phase cycle budget it was derived from is in
-// profiles/r02_rollout_phase_budget.txt): one CTA (256 threads = 8 warps) owns one instance for its whole episode.
+// Design: one CTA (256 threads = 8 warps) owns one instance for its whole episode.
 //   * warp h holds head h of glimpse_key, glimpse_val AND of the folded logit key (logit_key @ project_out, so that
 //     logits = sum_h o_h . L'_h[n]) for all nodes IN REGISTERS as float2 pairs (lane l owns nodes SPL*l .. SPL*l+SPL-1)
-//     and uses Blackwell's packed FFMA2.  Glimpse AND the head's share of every pointer logit are warp-local: one
+//     and keeps its FMAs in float2 pairs.  Glimpse AND the head's share of every pointer logit are warp-local: one
 //     REDUX.MAX on an order-preserving integer key, one shared-memory transpose for the value reduction, a 16-float
 //     broadcast of the un-normalised head output, and the 1/sum(exp) normalisation applied to the SPL partial logits
-//     (its shuffle reduction hides under the FFMA2s).  The version before read all 128 head outputs back per thread
-//     (16 LDS.128 per warp-step, LSU-bound: 318 of 2 160 cycles per selection); now a warp reads 4.
+//     (its shuffle reduction hides under the FMAs).  A warp reads 4 LDS.128 of head outputs per step; reading all 128
+//     head outputs back per thread would cost 16 and make the step LSU-bound.
 //   * barrier 1; thread n < NS sums the eight per-head partials of node n, tanh-clip, mask, temperature; the warp's
 //     arg-max is REDUX.MAX + ballot (lowest node wins ties, torch semantics); sampling = arg-max of z - log q
 //     (Gumbel form of torch.multinomial's p/q); barrier 2; every thread merges the <= 4 per-warp winners.
@@ -75,7 +74,6 @@ struct Smem {
   alignas(16) float pwk[32 * SPL * 8 + 8];    // ptab[n] . wk_h per (node, head); last 8 = the zero row
 };
 
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
 __device__ __forceinline__ float ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -306,7 +304,7 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
     }
     if (!(A.flags & CO_ROLLOUT_NO_PREFETCH) && b + (int)gridDim.x < B_inst) {  // next instance's cache rows -> L2
       // only the four blocks the kernel reads (K, V, L', current-node table): with the 5E layout the first-node table
-      // block would otherwise be pulled from HBM for nothing (measured: 1.24x the algorithmic DRAM traffic)
+      // block would otherwise be pulled from HBM for nothing
       const char* nxt = reinterpret_cast<const char*>(A.cache + (size_t)(b + gridDim.x) * N * CW);
       for (int i = tid; i < N * 16; i += 256) {  // 16 lines of 128 B per node row
         const int n = i >> 4, blk = (i >> 2) & 3, line = i & 3;
@@ -566,7 +564,7 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
               olh = fmaf(x.x, w.x, olh); olh = fmaf(x.y, w.y, olh); olh = fmaf(x.z, w.z, olh); olh = fmaf(x.w, w.w, olh);
             }
           }
-          esum = warp_sum_fixed(esum);  // 0 <= e <= 1 per node: two REDUX.SUM, independent of the FFMA2 block above
+          esum = warp_sum_fixed(esum);  // 0 <= e <= 1 per node: two REDUX.SUM, independent of the FMA block above
           const float rinv = __fdividef(1.0f, esum);
           float pl[SPL];
 #pragma unroll

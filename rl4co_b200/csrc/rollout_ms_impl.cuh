@@ -5,8 +5,8 @@
 // Same numerics as rollout_impl.cuh (read that header first); structure:
 //   * every phase handles the Q trajectories of the group before the block barrier, written
 //     stage-major in straight-line code so that their independent instruction streams interleave
-//     (a warp issues in order: a per-trajectory loop would serialise the chains and gain nothing --
-//     measured); the two barriers and the serial REDUX / MUFU / shuffle / LDS latencies are thereby
+//     (a warp issues in order: a per-trajectory loop would serialise the chains and gain nothing);
+//     the two barriers and the serial REDUX / MUFU / shuffle / LDS latencies are thereby
 //     amortised over Q node selections;
 //   * glimpse_key / glimpse_val head slices live in registers (warp h = head h, lane l owns nodes l + 32 k);
 //     the folded logit key lives in shared memory HEAD-MAJOR ([head][16-byte chunk][node], conflict-free

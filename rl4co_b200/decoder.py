@@ -17,8 +17,7 @@ What differs is the cache layout.  ``_precompute_cache`` does ONE GEMM
                                         row per start, a single-start episode one row.  `first_table=
                                         False` (CO_TSP_FIRST_TABLE=0) leaves the block out and the
                                         kernel does one 128x128 GEMV per episode instead: 20 % less GEMM
-                                        output, but measured 1.1 ms SLOWER per 65 536 x 100 step
-                                        (GEMM -1.4 ms, rollout kernel +2.5 ms), so it is not the default]
+                                        output for more work in the rollout kernel]
     last  embeddings @ Wctx_cur^T      current-node part of project_context (tsp: columns E:2E,
                                         cvrp: columns 0:E)
 
@@ -141,7 +140,7 @@ class FusedAttentionModelDecoder(nn.Module):
         self.project_fixed_context = nn.Linear(embed_dim, embed_dim, bias=False)
         self.use_graph_context = use_graph_context
         self.check_nan = check_nan
-        #: "tf32x3": hand-written tcgen05 3xTF32 GEMM (fp32-class accuracy, inference / no-grad only);
+        #: "tf32x3": hand-written wgmma 3xTF32 GEMM (fp32-class accuracy, inference / no-grad only);
         #: "cublas": torch.nn.functional.linear (strict fp32 SIMT; always used when autograd is on)
         self.cache_gemm = cache_gemm
 

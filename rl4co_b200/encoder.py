@@ -9,8 +9,8 @@ with the reference's module tree so that a reference ``state_dict`` loads unchan
   MLP                     rl4co/models/nn/mlp.py:8-60
 
 It runs once per instance.  Inference (no autograd, eval mode, CUDA): every nn.Linear runs on the
-hand-written tcgen05 3xTF32 GEMM (`co_gemm_tf32x3`; bias / ReLU / skip connection / eval-mode
-BatchNorm folded into its epilogue) and the attention core on `co_encoder_mha` (tcgen05 scores
+hand-written wgmma 3xTF32 GEMM (`co_gemm_tf32x3`; bias / ReLU / skip connection / eval-mode
+BatchNorm folded into its epilogue) and the attention core on `co_encoder_mha` (wgmma scores
 and P.V for N > 64), the FFN block on `co_ffn_fused`, instance normalisation on `co_instance_norm`
 -- `_net_fused` below.  Still stock torch ops there: the K = 2 / 3 init embedding and the
 graph-context mean + Linear of the decoder.  Under autograd (training) the stock Linear / norm modules
@@ -177,7 +177,7 @@ class AttentionModelEncoder(nn.Module):
     #: instances per forward chunk when no autograd graph is needed (bounds the FFN-hidden
     #: activation to chunk * N * 512 floats; exact because eval-mode norms are per element)
     inference_chunk = 65536
-    #: "tf32x3": Linear layers run on the hand-written tcgen05 3xTF32 GEMM (fp32-class accuracy)
+    #: "tf32x3": Linear layers run on the hand-written wgmma 3xTF32 GEMM (fp32-class accuracy)
     #: with bias / ReLU / skip connection / eval-mode BatchNorm folded into its epilogue -- CUDA,
     #: no-grad, eval only; "cublas": stock nn.Linear (strict fp32), always used under autograd.
     gemm = "tf32x3"
@@ -302,7 +302,7 @@ class AttentionModelEncoder(nn.Module):
             aff = self._bn_affine(norm2)
             if self._ffn_fusable(ffn):
                 # FF1 -> ReLU -> FF2 (+ skip, + folded BatchNorm) in one kernel: the [B*N, 512] hidden activation
-                # stays in tensor memory (co_ffn_fused); CO_FFN=split forces the separate GEMMs
+                # stays in registers (co_ffn_fused); CO_FFN=split forces the separate GEMMs
                 h = native.ffn_fused(h, self._ffn_tiled(lins[0].weight, lins[1].weight), lins[0].bias, lins[1].bias,
                                      scale=aff[0] if aff is not None else None, shift=aff[1] if aff is not None else None)
                 if aff is None:

@@ -21,9 +21,9 @@ CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 LIB_PATH = os.path.join(_HERE, "libcorollout.so")
 SOURCES = ["abi.cu", "env_kernels.cu", "decode_step.cu", "rollout.cu", "rollout_tsp.cu", "rollout_cvrp.cu", "rollout_ms_tsp.cu", "rollout_ms_cvrp.cu", "rollout_sdvrp.cu", "rollout_op.cu", "rollout_pctsp.cu", "gemm_tf32x3.cu",
-           "encoder_mha.cu", "encoder_mha_tc.cu", "encoder_mha_tc2.cu", "encoder_mha_tc3.cu",
+           "encoder_mha.cu", "encoder_mha_wgmma.cu",
            "ffn_fused.cu", "data_kernels.cu", "attn_train.cu", "norm_kernels.cu", "op_kernels.cu"]
-HEADERS = ["co_common.cuh", "rollout_impl.cuh", "rollout_ms_impl.cuh"]
+HEADERS = ["co_common.cuh", "rollout_impl.cuh", "rollout_ms_impl.cuh", "wgmma.cuh"]
 
 CO_OK = 0
 ENV_TSP, ENV_CVRP = 0, 1
@@ -77,7 +77,7 @@ class AttnArgs(Structure):
                 + [("scale", c_float)])
 
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-I", INCLUDE]
 
 
@@ -87,7 +87,7 @@ def _nvcc() -> str:
 
 
 def build(force: bool = False, verbose: bool = False, extra_flags: list[str] | None = None) -> str:
-    """Compile libcorollout.so in-tree for sm_100a (nvcc cross-compiles without a GPU).
+    """Compile libcorollout.so in-tree for sm_90a (nvcc cross-compiles without a GPU).
     Translation units are compiled in parallel, then linked."""
     deps = [os.path.join(CSRC, s) for s in SOURCES + HEADERS] + [os.path.join(INCLUDE, "corollout.h")]
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(s) for s in deps):
@@ -108,7 +108,7 @@ def build(force: bool = False, verbose: bool = False, extra_flags: list[str] | N
         if p.returncode != 0:
             raise NativeLibraryError(f"nvcc failed on {s} ({p.returncode}):\n{out}")
         objs.append(obj)
-    link = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB_PATH] + objs
+    link = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB_PATH] + objs
     res = subprocess.run(link, capture_output=True, text=True)
     if res.returncode != 0:
         raise NativeLibraryError(f"link failed ({res.returncode}):\n{res.stdout}\n{res.stderr}")
@@ -414,7 +414,7 @@ def split_tf32(w: torch.Tensor):
 
 @_on_device_of_first_tensor
 def gemm_tf32x3(a, w_hi, w_lo, out=None, bias=None, residual=None, scale=None, shift=None, relu=False):
-    """out[M, Nout] = epilogue(a[M, K] @ W[Nout, K]^T) on tcgen05 tensor cores (3xTF32).
+    """out[M, Nout] = epilogue(a[M, K] @ W[Nout, K]^T) on wgmma tensor cores (3xTF32).
     `a`, `out`, `residual` may be row-strided 2-D views (unit column stride)."""
     M, K = a.shape
     Nout = w_hi.shape[0]

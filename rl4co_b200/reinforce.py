@@ -295,7 +295,7 @@ class RolloutBaseline(NoBaseline):
         self._update_policy(policy, env, batch_size, device, dataset_size, dataset)
 
     def update(self, policy):
-        """Swap the frozen copy without touching the evaluation dataset (kept from round 1)."""
+        """Swap the frozen copy without touching the evaluation dataset."""
         self.policy = copy.deepcopy(policy).eval()
         for p in self.policy.parameters():
             p.requires_grad_(False)

@@ -11,13 +11,13 @@ if ROOT not in sys.path:
 
 GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
-# the CPU oracle works on [B, N, 128]-sized tensors: torch's default of one thread per core is ~14x slower than 16
-# threads on the 128-core GPU hosts (measured in bench.py's thread probe)
+# the CPU oracle works on [B, N, 128]-sized tensors: torch's default of one thread per core is far slower than 16
+# threads on a many-core host
 torch.set_num_threads(min(16, os.cpu_count() or 1))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

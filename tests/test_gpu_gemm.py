@@ -1,4 +1,4 @@
-"""GPU: tcgen05 3xTF32 GEMM (co_gemm_tf32x3) against a float64 reference; accuracy must be
+"""GPU: wgmma 3xTF32 GEMM (co_gemm_tf32x3) against a float64 reference; accuracy must be
 fp32-class (a plain TF32 GEMM would be ~1e-3 relative and fail)."""
 
 import pytest
@@ -69,10 +69,10 @@ def test_gemm_strided_views_and_column_block_output():
     assert (outbuf[:, :128] == 0).all() and (outbuf[:, 384:] == 0).all()
 
 
-@pytest.mark.parametrize("M", [1, 127, 128, 129, 1000, 148 * 128 + 77, 40000])
+@pytest.mark.parametrize("M", [1, 127, 128, 129, 1000, 132 * 128 + 77, 148 * 128 + 77, 40000])
 @pytest.mark.parametrize("affine", [True, False])
 def test_ffn_fused_vs_float64(M, affine):
-    """co_ffn_fused (FF1 -> ReLU -> FF2 + skip + folded BatchNorm, hidden activation in tensor memory) against a
+    """co_ffn_fused (FF1 -> ReLU -> FF2 + skip + folded BatchNorm, hidden activation in registers) against a
     float64 evaluation of SkipConnection(MLP) + eval BatchNorm (nn/graph/attnnet.py:33-53).  M = 40 000 makes the
     persistent CTAs loop over several tiles (weight ring / accumulator phase wrap-around)."""
     from rl4co_b200 import native

@@ -1,4 +1,4 @@
-"""GPU-vs-GPU comparator (SURVEY.md 8d): the reference ALGORITHM in PyTorch eager on the B200
+"""GPU-vs-GPU comparator (SURVEY.md 8d): the reference ALGORITHM in PyTorch eager on the GPU
 (the oracle port, fp32, TF32 off, host syncs and per-step K/V/L copies as in rl4co) next to the fused
 path on the same instances.  Test/bench infrastructure: imports oracle/."""
 import json, os, sys, time

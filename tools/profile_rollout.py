@@ -14,7 +14,7 @@ from rl4co_b200.policy import FusedAttentionModelPolicy
 p = argparse.ArgumentParser()
 p.add_argument("--env", default="tsp")
 p.add_argument("--num-loc", type=int, default=100)
-p.add_argument("--batch", type=int, default=148 * 8)
+p.add_argument("--batch", type=int, default=132 * 8)
 p.add_argument("--iters", type=int, default=3)
 p.add_argument("--decode-type", default="greedy")
 p.add_argument("--num-starts", type=int, default=0)

@@ -1,13 +1,12 @@
 """Driver for ncu / timing of the eight step-at-a-time kernels at the BASELINE size (65 536 x 100):
 three full env.step / decoder.forward / strategy.step rounds through the public stepping API, then reward +
-validity + baseline statistics.  Also prints CUDA-event times and the achieved fraction of the HBM copy
-bandwidth per kernel (algorithmic bytes of DESIGN.md 4.2 / kernel time), so the same script gives the numbers
+validity + baseline statistics.  Also prints CUDA-event times and the achieved fraction of the data-sheet HBM
+bandwidth per kernel (algorithmic bytes / kernel time), so the same script gives the numbers
 with and without the profiler (a time taken under ncu is never a bench value).
 
     python tools/profile_stepping.py [--batch 65536] [--num-loc 100]
 """
 import argparse
-import json
 import os
 import sys
 
@@ -25,10 +24,7 @@ p.add_argument("--num-loc", type=int, default=100)
 p.add_argument("--rounds", type=int, default=3)
 a = p.parse_args()
 dev = torch.device("cuda:0")
-try:
-    PEAK = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"]
-except Exception:
-    PEAK = 6650.0
+PEAK = 3350.0  # HBM3 bandwidth of the H100 SXM in GB/s (NVIDIA data sheet), as in bench.py
 
 
 def timed(fn, n=5):

@@ -1,6 +1,5 @@
 """SASS opcode histogram of the shipped library (no GPU needed): proves which hardware paths the kernels use
-(UTCHMMA / UTCBAR / LDTM / STTM = tcgen05 + TMEM, UTMALDG / UTMASTG = TMA, FFMA2 = packed FP32, CREDUX = warp
-reductions, LDGSTS = cp.async).  usage: python tools/sass_histogram.py [lib.so] > profiles/rNN_sass_histogram.txt"""
+(HGMMA = wgmma, UBLKCP = TMA bulk copy, SYNCS = mbarrier, REDUX = warp reductions, LDGSTS = cp.async).  usage: python tools/sass_histogram.py [lib.so] > sass_histogram.txt"""
 import collections
 import re
 import subprocess
@@ -20,15 +19,14 @@ for line in out.splitlines():
         op = m.group(1)
         per_kernel[cur][op] += 1
         total[op] += 1
-KEY = ["UTCHMMA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "UTCCP", "UTMALDG", "UTMASTG", "LDGSTS", "FFMA2", "FADD2", "FMUL2",
-       "CREDUX", "REDUX", "MUFU", "SHFL", "LDS", "STS", "BAR", "SYNCS", "FFMA", "HMMA", "ATOMS", "LDL", "STL"]
-print(f"# {lib}: {sum(total.values())} SASS instructions in {len(per_kernel)} kernels (sm_100a)")
+KEY = ["HGMMA", "WARPGROUP", "UBLKCP", "UTMALDG", "UTMASTG", "LDGSTS", "SYNCS", "REDUX", "MUFU", "SHFL", "LDS", "STS", "BAR", "FFMA", "HMMA", "ATOMS", "LDL", "STL"]
+print(f"# {lib}: {sum(total.values())} SASS instructions in {len(per_kernel)} kernels (sm_90a)")
 print("## whole library, selected opcodes")
 for k in KEY:
     print(f"  {k:10s} {total.get(k, 0)}")
-print("## per kernel (kernels with tensor-core / TMEM / async-copy / packed-FP32 instructions)")
+print("## per kernel (kernels with tensor-core / bulk-copy / async-copy / warp-reduction instructions)")
 for name, c in sorted(per_kernel.items()):
     sel = {k: c[k] for k in KEY if c.get(k)}
-    if any(k in sel for k in ("UTCHMMA", "LDTM", "STTM", "UTMALDG", "LDGSTS", "FFMA2", "CREDUX")):
+    if any(k in sel for k in ("HGMMA", "UBLKCP", "UTMALDG", "LDGSTS", "REDUX")):
         print(f"  {name[:100]}")
         print("     " + "  ".join(f"{k}={v}" for k, v in sel.items()))
