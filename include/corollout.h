@@ -128,6 +128,23 @@ int co_check_tours(const int64_t* actions, const float* demand,
                    const float* vehicle_capacity, int32_t* bad_count, int B, int B_inst,
                    int N, int T, void* stream);
 
+/* TSPEnv.local_search  (rl4co/envs/routing/tsp/env.py:184-188 -> tsp/local_search.py)
+ *   best-improvement 2-opt with position 0 fixed, bit-identical to the reference: per sweep the first pair (i, j) in
+ *   loop order with the smallest fp32 change below -1e-6 has t[i..j] reversed; sweeps repeat until none improves or
+ *   max_iterations sweeps have run (<= 0: tours copied unchanged).
+ *   Distances: exactly one of
+ *     locs [B,N,2]  -> d[a,b] = sqrt(fma(dy, dy, dx*dx)), dx = x_a - x_b (get_distance_matrix on the CPU), or
+ *     dist [B,N,N]  -> used as given, possibly asymmetric;
+ *   the diagonal gets +1e9 in both cases.  The matrix is held in shared memory up to CO_TWO_OPT_RESIDENT_MAX_NODES
+ *   nodes (locs: computed there), above that read through L2 (dist) or computed per read from locs.
+ *   tours_in / tours_out [B,N] int64, and tours_out may alias tours_in.  A tour holding an id outside [0, N) is
+ *   copied through unchanged with iterations[b] = -1.  iterations [B] (nullable) receives the number of sweeps run.
+ *   N > CO_TWO_OPT_MAX_NODES returns CO_ERR_UNSUPPORTED. */
+#define CO_TWO_OPT_MAX_NODES 1024
+#define CO_TWO_OPT_RESIDENT_MAX_NODES 224 /* 224*224*4 B = 196 KiB of the 227 KiB a CTA may use */
+int co_tsp_two_opt(const float* locs, const float* dist, const int64_t* tours_in, int64_t* tours_out,
+                   int32_t* iterations, int B, int N, int max_iterations, void* stream);
+
 /* ------------------------------------------------------------------ decoder, one step */
 
 /* Weights of the decoder path, device pointers, all float32, no biases

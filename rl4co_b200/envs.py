@@ -252,6 +252,10 @@ class FusedEnvBase:
     def select_start_nodes(self, td, num_starts):
         return select_start_nodes(td, self, num_starts)
 
+    def local_search(self, td: TensorDict, actions: torch.Tensor, **kwargs) -> torch.Tensor:
+        """rl4co/envs/common/base.py:228-232"""
+        raise NotImplementedError(f"Local is not implemented yet for {self.name} environment")
+
     def dataset(self, batch_size=[], phase="train", filename=None):
         """rl4co/envs/common/base.py:234-268: the phase's file (`{phase}_file`, or `filename`) when set -- e.g. the
         seeded validation / test sets of data.generate_default_datasets -- else freshly generated instances; a
@@ -343,6 +347,30 @@ class FusedTSPEnv(FusedEnvBase):
         """tsp/env.py:158-164"""
         bad = native.check_tours(actions.contiguous(), td["locs"].shape[-2])
         assert bad == 0, "Invalid tour"
+
+    @staticmethod
+    def local_search(td: TensorDict, actions: torch.Tensor, max_iterations: int = 1000,
+                     num_threads: int | None = None) -> torch.Tensor:
+        """tsp/env.py:184-188 -> tsp/local_search.py: best-improvement 2-opt of `actions` [B, N] (position 0 fixed) in
+        one kernel (co_tsp_two_opt), tour for tour what the reference's numba 2-opt returns.  Distances are
+        td["distances"] (float32 [B, N, N], used as given) when present, else those of td["locs"].  `num_threads`
+        (the reference's host thread count) is accepted and ignored.  Returns a new int64 tensor on actions.device."""
+        del num_threads
+        if len(td.batch_size) > 1:
+            raise ValueError(f"local_search takes a batch with one dimension, got batch_size {tuple(td.batch_size)}")
+        distances = td.get("distances", None)
+        src = td["locs"] if distances is None else distances
+        if distances is not None and distances.dtype != torch.float32:
+            raise ValueError(f"distances must be float32, got {distances.dtype}")
+        B, N = src.shape[0], src.shape[-2]
+        if actions.dim() != 2 or tuple(actions.shape) != (B, N):
+            raise ValueError(f"actions must be [{B}, {N}] (one tour over every node), got {tuple(actions.shape)}")
+        tours = actions.to(device=src.device, dtype=torch.int64).contiguous()
+        if distances is None:
+            out = native.tsp_two_opt(tours, max_iterations, locs=src.to(torch.float32).contiguous())
+        else:
+            out = native.tsp_two_opt(tours, max_iterations, distances=distances.contiguous())
+        return out.to(actions.device)
 
 
 class FusedCVRPEnv(FusedEnvBase):

@@ -22,7 +22,7 @@ INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 LIB_PATH = os.path.join(_HERE, "libcorollout.so")
 SOURCES = ["abi.cu", "env_kernels.cu", "decode_step.cu", "rollout.cu", "rollout_tsp.cu", "rollout_cvrp.cu", "rollout_ms_tsp.cu", "rollout_ms_cvrp.cu", "rollout_sdvrp.cu", "rollout_op.cu", "rollout_pctsp.cu", "gemm_tf32x3.cu",
            "encoder_mha.cu", "encoder_mha_wgmma.cu",
-           "ffn_fused.cu", "data_kernels.cu", "attn_train.cu", "norm_kernels.cu", "op_kernels.cu"]
+           "ffn_fused.cu", "data_kernels.cu", "attn_train.cu", "norm_kernels.cu", "op_kernels.cu", "local_search.cu"]
 HEADERS = ["co_common.cuh", "rollout_impl.cuh", "rollout_ms_impl.cuh", "wgmma.cuh"]
 
 CO_OK = 0
@@ -42,6 +42,7 @@ EXPORTS = [
     "co_cache_width", "co_rollout_max_nodes", "co_rollout", "co_reward_stats", "co_split_tf32", "co_gemm_tf32x3", "co_encoder_mha",
     "co_ffn_fused", "co_ffn_tile_weights", "co_ffn_tiled_weight_floats", "co_generate_uniform", "co_generate_demand", "co_dihedral8",
     "co_sdvrp_step", "co_sdvrp_action_mask", "co_attn_fwd", "co_attn_bwd", "co_instance_norm", "co_op_step", "co_op_action_mask", "co_op_reward", "co_pctsp_step", "co_pctsp_action_mask",
+    "co_tsp_two_opt",
 ]
 
 
@@ -143,6 +144,7 @@ def lib() -> ctypes.CDLL:
     L.co_sdvrp_action_mask.argtypes = [c_void_p] * 5 + [c_int, c_int, c_void_p]
     L.co_sdvrp_step.argtypes = [c_void_p] * 9 + [c_int, c_int, c_void_p]
     L.co_check_tours.argtypes = [c_void_p] * 4 + [c_int] * 4 + [c_void_p]
+    L.co_tsp_two_opt.argtypes = [c_void_p] * 5 + [c_int] * 3 + [c_void_p]
     L.co_reward_stats.argtypes = [c_void_p, c_void_p, c_int, c_void_p]
     L.co_op_action_mask.argtypes = [c_void_p] * 6 + [c_int, c_int, c_void_p]
     L.co_op_step.argtypes = [c_void_p] * 12 + [c_int, c_int, c_void_p]
@@ -363,6 +365,29 @@ def check_tours(actions, N, demand=None, cap=None, B_inst=None) -> int:
                                 _ptr(bad, I32, "bad"), B, B if B_inst is None else B_inst, N, T, _stream()),
            "co_check_tours")
     return int(bad.item())
+
+
+@_on_device_of_first_tensor
+def tsp_two_opt(tours, max_iterations: int = 1000, locs=None, distances=None, iterations=None):
+    """co_tsp_two_opt (tsp/local_search.py): 2-opt of int64 tours [B, N] with position 0 fixed -> new [B, N] int64.
+    Exactly one of `locs` [B, N, 2] / `distances` [B, N, N] (float32) gives the distances; `iterations` is an optional
+    int32 [B] output (sweeps run per instance, -1 for a tour with an id outside [0, N))."""
+    if (locs is None) == (distances is None):
+        raise ValueError("tsp_two_opt: pass exactly one of locs / distances")
+    if tours.dim() != 2:
+        raise ValueError(f"tours: expected [B, N], got {tuple(tours.shape)}")
+    B, N = tours.shape
+    if locs is not None and tuple(locs.shape) != (B, N, 2):
+        raise ValueError(f"locs: expected [{B}, {N}, 2], got {tuple(locs.shape)}")
+    if distances is not None and tuple(distances.shape) != (B, N, N):
+        raise ValueError(f"distances: expected [{B}, {N}, {N}], got {tuple(distances.shape)}")
+    if iterations is not None and tuple(iterations.shape) != (B,):
+        raise ValueError(f"iterations: expected [{B}], got {tuple(iterations.shape)}")
+    out = torch.empty(B, N, dtype=I64, device=tours.device)
+    _check(lib().co_tsp_two_opt(_ptr(locs, F32, "locs"), _ptr(distances, F32, "distances"), _ptr(tours, I64, "tours"),
+                                _ptr(out, I64, "tours_out"), _ptr(iterations, I32, "iterations"), B, N,
+                                min(int(max_iterations), 2**31 - 1), _stream()), "co_tsp_two_opt")
+    return out
 
 
 @_on_device_of_first_tensor

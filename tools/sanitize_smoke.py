@@ -58,3 +58,15 @@ AT.self_attention_packed(qkv).sum().backward()
 native.instance_norm(torch.randn(9, 100, 128, device=dev), torch.ones(128, device=dev), torch.zeros(128, device=dev))
 torch.cuda.synchronize()
 print("attention / norm ok")
+# 2-opt local search (co_tsp_two_opt): both distance sources, on both sides of the shared-memory residency bound
+# (CO_TWO_OPT_RESIDENT_MAX_NODES = 224); the in-place segment reversal is what racecheck looks at
+for n in (20, 224, 300):
+    g = torch.Generator().manual_seed(n)
+    locs = torch.rand(4, n, 2, generator=g).to(dev)
+    tours = torch.argsort(torch.rand(4, n, generator=g), dim=1).to(dev)
+    d = (locs[:, :, None] - locs[:, None]).norm(dim=-1)
+    its = torch.empty(4, dtype=torch.int32, device=dev)
+    native.tsp_two_opt(tours, 50, locs=locs, iterations=its)
+    native.tsp_two_opt(tours, 50, distances=d, iterations=its)
+torch.cuda.synchronize()
+print("local search ok")
