@@ -133,7 +133,7 @@ def test_op_policy_vs_golden(golden, name, mode, fused, monkeypatch):
     torch.testing.assert_close(out["reward"].cpu()[same], rr[same], rtol=RTOL, atol=1e-6)
 
 
-@pytest.mark.parametrize("n,batch", [(20, 64), (100, 32)])
+@pytest.mark.parametrize("n,batch", [(20, 64), (100, 32), (31, 48), (64, 32), (127, 16)])
 def test_op_policy_vs_oracle_on_fresh_instances(n, batch):
     """Seeded fresh instances (on-device generator off: the CPU call order): teacher-forced oracle log-probs / rewards of
     the GPU's own greedy and sampled actions, valid tours (check_solution=True); multistart decoding runs (its forced

@@ -392,7 +392,8 @@ def test_stepping_path_beam_search_vs_oracle(golden, dev, name, beam_width, sele
 # ------------------------------------------------------------------------------- bigger seeded cases
 @pytest.mark.parametrize("env_name,n,batch", [("tsp", 100, 96), ("cvrp", 100, 96), ("tsp", 50, 128), ("cvrp", 50, 128),
                                               ("tsp", 7, 33), ("cvrp", 5, 33), ("tsp", 128, 16), ("cvrp", 127, 16),
-                                              ("tsp", 33, 40), ("cvrp", 64, 40)])
+                                              ("tsp", 33, 40), ("cvrp", 64, 40), ("tsp", 2, 33), ("tsp", 32, 40),
+                                              ("tsp", 64, 40), ("cvrp", 31, 40), ("cvrp", 32, 40), ("cvrp", 63, 40)])
 @pytest.mark.parametrize("mode", ["greedy", "sampling"])
 def test_full_policy_vs_oracle_seeded(dev, env_name, n, batch, mode):
     """Encoder + cache + persistent rollout vs the CPU oracle on seeded instances at the
@@ -654,10 +655,12 @@ def test_philox_sampling_distribution_step_kernel(dev):
         assert chi2 < 45.0, f"chi2 {chi2:.1f} with {dof} dof (p < 1e-5 at 45 for 9 dof)"  # 9 dof: 99.999 % quantile 37.3
 
 
-@pytest.mark.parametrize("env_name", ["tsp", "cvrp"])
-def test_philox_sampling_distribution_rollout_kernel(dev, env_name):
-    """The persistent kernel's Gumbel-form sampling (arg-max of z - log q, q = Philox Exp(1)): B copies of ONE
-    instance, the first free selection of every copy must follow the kernel's own reported distribution."""
+@pytest.mark.parametrize("env_name,temperature", [("tsp", 1.0), ("cvrp", 1.0), ("tsp", 2.0), ("cvrp", 2.0)],
+                         ids=["tsp", "cvrp", "tsp-T2", "cvrp-T2"])
+def test_philox_sampling_distribution_rollout_kernel(dev, env_name, temperature):
+    """The persistent kernel's Gumbel-form sampling (arg-max of z - log q, q = Philox Exp(1), z divided by the
+    temperature): B copies of ONE instance, the first free selection of every copy must follow the kernel's own
+    reported distribution."""
     from rl4co_b200.envs import get_env
     from rl4co_b200.policy import FusedAttentionModelPolicy
     from rl4co_b200.tensordict import TensorDict
@@ -673,7 +676,7 @@ def test_philox_sampling_distribution_rollout_kernel(dev, env_name):
     td_host = TensorDict({k: one[k].expand(B, *one[k].shape[1:]).contiguous() for k in one.keys()}, batch_size=[B])
     with torch.inference_mode():
         td = env.reset(td_host.to(dev))
-        out = pol(td, env, decode_type="sampling", seed=21, return_sum_log_likelihood=False)
+        out = pol(td, env, decode_type="sampling", seed=21, temperature=temperature, return_sum_log_likelihood=False)
     a0, lp0 = out["actions"][:, 0].cpu(), out["log_likelihood"][:, 0].cpu().double()
     N = td["action_mask"].shape[-1]
     counts = torch.bincount(a0, minlength=N).double()

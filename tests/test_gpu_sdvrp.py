@@ -136,7 +136,7 @@ def test_sdvrp_policy_vs_golden(golden, name, mode, fused, monkeypatch):
 
 
 @pytest.mark.parametrize("fused", [True, False])
-@pytest.mark.parametrize("n,batch", [(20, 64), (50, 64), (100, 32), (5, 40)])
+@pytest.mark.parametrize("n,batch", [(20, 64), (50, 64), (100, 32), (5, 40), (31, 48), (64, 32), (127, 16)])
 def test_sdvrp_policy_vs_prefix_oracle(n, batch, fused):
     """Seeded larger cases: every GPU choice is the oracle's (near-)best for the same prefix, log-probs / reward
     agree, tours are valid."""
