@@ -287,9 +287,10 @@ def sdvrp_check_solution(st, actions):
 def sdvrp_dynamic_embedding(weights, st):
     """nn/env_embeddings/dynamic.py:60-78 (SDVRPDynamicEmbedding): Linear(1 -> 3E, no bias) of the remaining demand,
     depot entry forced to 0; chunks add to glimpse_key / glimpse_val / logit_key (am/decoder.py:142-154)."""
-    d = st["demand_with_depot"][..., None].clone()
+    w = _w(weights, "dynamic_embedding.projection.weight")
+    d = st["demand_with_depot"][..., None].to(w.dtype, copy=True)  # the env state stays fp32; the network runs in the weights' dtype
     d[..., 0, :] = 0
-    return F.linear(d, _w(weights, "dynamic_embedding.projection.weight")).chunk(3, dim=-1)
+    return F.linear(d, w).chunk(3, dim=-1)
 
 
 # reference: rl4co/envs/routing/op/env.py (orienteering: collect prizes, return to the depot within max_length)
@@ -722,6 +723,36 @@ def rollout(weights, env_name, inst, h, decode_type="greedy", num_starts=None, a
     return out
 
 
+def teacher_forced_logprobs(weights, env_name, inst, h, acts, num_starts=1, forced_first=False, temperature=1.0,
+                            tanh_clipping=10.0, use_graph_context=True):
+    """Per-step log-probabilities [B*S, T] of given trajectories ``acts`` [B*S, T], differentiable in ``weights`` and
+    ``h`` (no inference mode; float64 weights and ``h`` give a float64 network over the fp32 env state).
+
+    The decode loop of constructive/base.py:209-251 teacher-forced step by step. S > 1 rows are start-major over the
+    batchified instances (flat index s * B + b). ``forced_first``: the first action is a forced multistart start taken
+    by the env step without a decoder call, with log-prob 0 (decoding.py:309-326); ``rollout(actions=...)`` would score
+    it. T is the oracle's episode length: columns of ``acts`` past it (the padding of finished trajectories) are not
+    read."""
+    if num_starts > 1:
+        inst, h = batchify(inst, num_starts), batchify(h, num_starts)
+    st = env_reset(env_name, inst)
+    step_fn = ENV_STEP[env_name]
+    cache = precompute_cache(weights, h, use_graph_context)
+    lps, t = [], 0
+    if forced_first:
+        st = step_fn(st, acts[:, 0])
+        lps.append(torch.zeros(acts.shape[0], dtype=h.dtype))
+        t = 1
+    while not st["done"].all():
+        assert t < acts.shape[1], "the trajectories end before the episode does"
+        logits, mask = decoder_forward(weights, env_name, st, cache, 0, faithful_copies=False)
+        lp = process_logits(logits.clone(), mask, temperature, tanh_clipping)
+        lps.append(lp.gather(1, acts[:, t:t + 1]).squeeze(1))
+        st = step_fn(st, acts[:, t])
+        t += 1
+    return torch.stack(lps, 1)
+
+
 # --------------------------------------------------------------------------- beam search
 # reference: rl4co/utils/decoding.py:464-600 (BeamSearch strategy) inside the loop of constructive/base.py:219-251
 
@@ -796,10 +827,13 @@ def rollout_beam_search(weights, env_name, inst, h, beam_width=None, select_best
 
 
 def init_embedding(weights, env_name, st):
+    """Raw instance data enters the network in the weights' dtype (float64 weights give a float64 network over the
+    fp32 env state)."""
     p = "encoder.init_embedding."
+    locs = st["locs"].to(weights[p + "init_embed.weight"].dtype)
     if env_name == "tsp":
-        return F.linear(st["locs"], weights[p + "init_embed.weight"], weights[p + "init_embed.bias"])
-    depot, cities = st["locs"][:, :1, :], st["locs"][:, 1:, :]
+        return F.linear(locs, weights[p + "init_embed.weight"], weights[p + "init_embed.bias"])
+    depot, cities = locs[:, :1, :], locs[:, 1:, :]
     de = F.linear(depot, weights[p + "init_embed_depot.weight"], weights[p + "init_embed_depot.bias"])
     feat = st["prize"][..., 1:, None] if env_name == "op" else None  # init.py:254-280 / 115-136
     if env_name == "pctsp":  # init.py:221-251: (x, y, expected prize, penalty)
@@ -810,18 +844,28 @@ def init_embedding(weights, env_name, st):
     return torch.cat((de, ne), -2)
 
 
-def _normalization(weights, prefix, x, kind):
+def _normalization(weights, prefix, x, kind, batch_stats=False):
+    """`batch_stats`: batch normalisation with the statistics of this batch (a module in train mode); the running
+    statistics are read otherwise, and never updated."""
     w, b = weights[prefix + "normalizer.weight"], weights[prefix + "normalizer.bias"]
-    if kind == "batch":  # eval mode: running stats
-        y = F.batch_norm(x.reshape(-1, x.size(-1)), weights[prefix + "normalizer.running_mean"],
-                         weights[prefix + "normalizer.running_var"], w, b, training=False, eps=1e-5)
+    if kind == "batch":
+        if batch_stats:
+            y = F.batch_norm(x.reshape(-1, x.size(-1)), None, None, w, b, training=True, eps=1e-5)
+        else:
+            y = F.batch_norm(x.reshape(-1, x.size(-1)), weights[prefix + "normalizer.running_mean"],
+                             weights[prefix + "normalizer.running_var"], w, b, training=False, eps=1e-5)
         return y.view(*x.size())
     if kind == "instance":
         return F.instance_norm(x.permute(0, 2, 1), weight=w, bias=b, eps=1e-5).permute(0, 2, 1)
     raise ValueError(kind)
 
 
-def encoder_forward(weights, env_name, st, num_layers=3, num_heads=8, normalization="batch"):
+def encoder_forward(weights, env_name, st, num_layers=3, num_heads=8, normalization="batch", batch_stats=False,
+                    relu_masks=None, pre_activations=None):
+    """``relu_masks``: one bool tensor per layer, the units of the FFN's ReLU to keep, in place of the sign of this
+    forward's own pre-activation. A gradient check uses the checked network's activation pattern: a unit whose
+    pre-activation lies within round-off of 0 may sit on either side in fp32, and the gradient jumps there.
+    ``pre_activations``: a list that receives each layer's ReLU input (detached)."""
     h = init_embedding(weights, env_name, st)
     init_h = h
     for i in range(num_layers):
@@ -832,10 +876,13 @@ def encoder_forward(weights, env_name, st, num_layers=3, num_heads=8, normalizat
         o = F.scaled_dot_product_attention(q, k, v)
         o = o.transpose(1, 2).reshape(B, N, -1)
         h = h + F.linear(o, weights[p + "0.module.out_proj.weight"], weights[p + "0.module.out_proj.bias"])
-        h = _normalization(weights, p + "1.", h, normalization)
-        f = F.relu(F.linear(h, weights[p + "2.module.lins.0.weight"], weights[p + "2.module.lins.0.bias"]))
+        h = _normalization(weights, p + "1.", h, normalization, batch_stats)
+        f = F.linear(h, weights[p + "2.module.lins.0.weight"], weights[p + "2.module.lins.0.bias"])
+        if pre_activations is not None:
+            pre_activations.append(f.detach())
+        f = F.relu(f) if relu_masks is None else f * relu_masks[i].to(f.dtype)
         h = h + F.linear(f, weights[p + "2.module.lins.1.weight"], weights[p + "2.module.lins.1.bias"])
-        h = _normalization(weights, p + "3.", h, normalization)
+        h = _normalization(weights, p + "3.", h, normalization, batch_stats)
     return h, init_h
 
 
@@ -867,6 +914,37 @@ def shared_baseline(reward, num_starts):
 def mean_baseline(reward):
     """baselines.py:75-81 (ExponentialBaseline first call / MeanBaseline): reward.mean()"""
     return reward.mean()
+
+
+def float64_weights(state_dict, trainable):
+    """float64 CPU copy of a policy's ``state_dict`` for gradient checks: the names in ``trainable`` become leaves that
+    require grad, the other floating-point entries (normalisation buffers) plain float64 tensors."""
+    out = {}
+    for k, v in state_dict.items():
+        v = v.detach().cpu()
+        out[k] = v.double().requires_grad_(k in trainable) if v.is_floating_point() else v
+    return out
+
+
+def gradient_errors(grads, weights, floor=1e-2):
+    """Per-parameter comparison of ``grads`` {name: gradient or None} with the ``.grad`` of the float64 leaves in
+    ``weights``. Returns (rel, zero):
+      rel  {name: ||g - g64|| / max(||g64||, floor * G)} (Frobenius; G = the norm of the whole float64 gradient; a
+           missing product gradient counts as zeros). The floor keeps directions the loss is (nearly) invariant to --
+           the bias of a Linear right before a normalisation has a float64 gradient of round-off size -- from turning
+           fp32 round-off into a meaningless relative error;
+      zero {name: ||g||} where the float64 gradient is None or exactly 0 (the loss does not reach the parameter)."""
+    ref = {k: weights[k].grad for k in grads}
+    total = math.sqrt(sum(float(g.square().sum()) for g in ref.values() if g is not None))
+    rel, zero = {}, {}
+    for k, g in grads.items():
+        g64 = ref[k]
+        if g64 is None or not bool(g64.any()):
+            zero[k] = 0.0 if g is None else float(g.detach().double().norm())
+            continue
+        diff = g64 if g is None else g.detach().double().cpu() - g64
+        rel[k] = float(diff.norm()) / max(float(g64.norm()), floor * total)
+    return rel, zero
 
 
 def pomo_reduce(reward, n_aug, n_start):

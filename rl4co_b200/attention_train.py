@@ -34,6 +34,12 @@ def pack_mask(mask: torch.Tensor) -> torch.Tensor:
     return by.contiguous().view(torch.int32)                                                  # [B, M, 4]
 
 
+def _like(o, dO):
+    """dO with o's strides (the kernels read both through one set of strides). `.contiguous()` is not enough: a size-1
+    batch dimension may carry any stride, e.g. the gradient slice of one 256-query chunk of a single instance."""
+    return dO if dO.stride() == o.stride() else torch.empty_like(o).copy_(dO)
+
+
 class _Attention(torch.autograd.Function):
     """o = softmax(q k^T / 4 [masked]) v per head; q [B, M, E], k / v [B, N, E] (last dim contiguous, any row / batch
     stride that is a multiple of 4 floats -- column views of the fused cache are fine), mask words or None."""
@@ -51,7 +57,7 @@ class _Attention(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dO):
         q, k, v, o, lse, mw = ctx.saved_tensors
-        dO = dO.contiguous()
+        dO = _like(o, dO)
         dq = torch.empty(q.shape, device=q.device, dtype=torch.float32)
         dk = torch.empty(k.shape, device=q.device, dtype=torch.float32)
         dv = torch.empty(v.shape, device=q.device, dtype=torch.float32)
@@ -75,7 +81,7 @@ class _SelfAttentionPacked(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dO):
         qkv, o, lse = ctx.saved_tensors
-        dO = dO.contiguous()
+        dO = _like(o, dO)
         dqkv = torch.empty_like(qkv)
         native.attn_bwd(qkv[..., :E], qkv[..., E:2 * E], qkv[..., 2 * E:], None, o, lse, dO,
                         dqkv[..., :E], dqkv[..., E:2 * E], dqkv[..., 2 * E:])

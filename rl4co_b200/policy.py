@@ -242,6 +242,20 @@ class FusedAttentionModelPolicy(nn.Module):
             tanh_clipping=kw.pop("tanh_clipping", self.tanh_clipping),
             mask_logits=kw.pop("mask_logits", self.mask_logits),
             store_all_logp=kw.pop("store_all_logp", return_entropy), **kw)
+        # the step kernels are forward-only: under autograd the log-probs of the decoded actions are recomputed by the
+        # differentiable teacher-forced pass, as on the fused path; what that pass cannot replay is refused
+        regrad = torch.is_grad_enabled() and hidden.requires_grad
+        if regrad:
+            refused = [name for name, on in (("top_k", strategy.top_k > 0), ("top_p", strategy.top_p > 0),
+                                             ("return_entropy", return_entropy),
+                                             ("store_all_logp", strategy.store_all_logp),
+                                             ("beam_search", decode_type == "beam_search"),
+                                             ("select_best", strategy.select_best),
+                                             ("mask_logits=False", not strategy.mask_logits)) if on]
+            if refused:
+                raise NotImplementedError(f"{', '.join(refused)} under autograd: the differentiable teacher-forced pass "
+                                          f"does not replay it; decode under torch.no_grad()")
+        td_reset = td.clone() if regrad else None  # the env steps below update the state they are given in place
         td, env, num_starts = strategy.pre_decoder_hook(td, env)
         td, env, cached = self.decoder.pre_decoder_hook(td, env, hidden, num_starts)
         step = 0
@@ -253,6 +267,13 @@ class FusedAttentionModelPolicy(nn.Module):
             if step > max_steps:
                 break
         logprobs, out_actions, td, env = strategy.post_decoder_hook(td, env)
+        if regrad:
+            from .reinforce import evaluate_log_likelihood
+
+            logprobs = evaluate_log_likelihood(self, td_reset, env, out_actions.contiguous(), hidden=hidden,
+                                               return_sum=False, temperature=strategy.temperature,
+                                               tanh_clipping=strategy.tanh_clipping,
+                                               forced_first=strategy.multistart and num_starts >= 1)
         if calc_reward:
             td.set("reward", env.get_reward(td, out_actions))
         out = {"reward": td["reward"],
