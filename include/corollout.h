@@ -304,6 +304,50 @@ int co_generate_demand(float* out, long n, uint64_t seed, uint64_t offset, int m
                        float capacity, void* stream);
 int co_dihedral8(const float* locs, float* out, long B, int N, void* stream);
 
+/* co_generate_locs: out [B, N, 2] float32 locations from one location law (envs/common/utils.py get_sampler and
+ * envs/common/distribution_utils.py), one CTA per instance.  Philox4x32-10 keyed by `seed` with the counter
+ * (instance, draw index, offset): row b is the same for every B > b, launch shape and GPU.
+ *   UNIFORM                 U(lo, hi)^2
+ *   CONSTANT                every coordinate = lo (the caller resolves a number c, "center" = (max - min) / 2 and
+ *                           "corner" = min)
+ *   NORMAL                  i.i.d. N(mean, std^2), not clamped
+ *   CLUSTER                 k = n_cluster centres U(0.2, 0.8)^2; the nodes form k contiguous blocks of floor(N/k),
+ *                           the first N mod k one longer; node ~ N(its block's centre, 0.07^2 I), clamped to [0, 1]
+ *   MIXED                   U(0, 1)^2, then floor(N/2) distinct nodes in random order are cut into k = n_cluster_mix
+ *                           segments (k - 1 of floor(N/(2k)), the last takes the rest) and segment i is redrawn from
+ *                           N(c_i, 0.07^2 I), c_i ~ U(0.2, 0.8)^2; clamped to [0, 1]
+ *   GAUSSIAN_MIXTURE        (num_modes, cdist) = (0, 0): U(0, 1)^2.  (1, 1): N((.5, .5), [[1, r], [r, 1]]), r ~ U(0, 1)
+ *                           per instance, shifted by the per-coordinate minimum, divided by the larger of the two
+ *                           ranges and centred with + (1 - max) / 2 per coordinate.  Otherwise: each node's mode
+ *                           uniform over num_modes, nodes stored grouped by ascending mode, a non-empty mode's centre
+ *                           U(0, cdist)^2, node ~ N(centre, I), then min-max scaled to [0, 1] per coordinate.
+ *   MIX_DISTRIBUTION        p ~ U(0, 1) per instance: MIXED if p <= 0.33, CLUSTER if p <= 0.66, else U(0, 1)^2
+ *   MIX_MULTI_DISTRIBUTIONS per instance one (num_modes, cdist) uniform over {(0,0), (1,1)} + {3,5,7} x {10,30,50}
+ * 1 <= N <= CO_LOCS_MAX_NODES; GAUSSIAN_MIXTURE other than (0, 0) and MIX_MULTI_DISTRIBUTIONS need N >= 2;
+ * n_cluster, n_cluster_mix >= 1 where used; anything else is CO_ERR_BAD_ARG.  `out` must be 8-byte aligned. */
+#define CO_LOCS_MAX_NODES 10000
+#define CO_LOCS_UNIFORM 0
+#define CO_LOCS_CONSTANT 1
+#define CO_LOCS_NORMAL 2
+#define CO_LOCS_CLUSTER 3
+#define CO_LOCS_MIXED 4
+#define CO_LOCS_GAUSSIAN_MIXTURE 5
+#define CO_LOCS_MIX_DISTRIBUTION 6
+#define CO_LOCS_MIX_MULTI_DISTRIBUTIONS 7
+typedef struct co_locs_args {
+  int64_t B;              /* instances */
+  int32_t N;              /* nodes per instance (depot included where there is one) */
+  int32_t kind;           /* CO_LOCS_* */
+  uint64_t seed, offset;  /* Philox key / stream */
+  float lo, hi;           /* UNIFORM range; CONSTANT value = lo */
+  float mean, std;        /* NORMAL */
+  int32_t n_cluster;      /* CLUSTER, MIX_DISTRIBUTION */
+  int32_t n_cluster_mix;  /* MIXED, MIX_DISTRIBUTION */
+  int32_t num_modes;      /* GAUSSIAN_MIXTURE */
+  float cdist;            /* GAUSSIAN_MIXTURE */
+} co_locs_args;
+int co_generate_locs(float* out, const co_locs_args* args, void* stream);
+
 /* Encoder self-attention core: F.scaled_dot_product_attention of MultiHeadAttention
  * (rl4co/models/nn/attention.py:110-134) on the packed projection qkv [B*N, 3E] ("three h d"),
  * 8 heads x 16, no mask, fp32 -> out [B*N, E] ("h d"); N <= 128. */

@@ -36,9 +36,10 @@ class Generator:
 
 class _DeviceStream:
     """On-device generation state: `device="cuda"` makes a generator write instances straight into HBM with
-    co_generate_uniform / co_generate_demand (Philox keyed by `seed`; every call advances `offset`, so successive
-    batches differ and a (seed, call index) pair always reproduces the same batch).  Default: torch's CPU
-    generator in the reference's call order (bit-identical to the reference under the same torch seed)."""
+    co_generate_uniform / co_generate_demand / co_generate_locs (Philox keyed by `seed`; every call advances `offset`,
+    so successive batches differ and a (seed, call index) pair always reproduces the same batch).  Default: torch's
+    CPU generator in the reference's call order (bit-identical to the reference under the same torch seed), which
+    serves uniform locations only."""
 
     def _init_stream(self, device, seed):
         self.device = None if device is None else torch.device(device)
@@ -54,32 +55,125 @@ class _DeviceStream:
         self.calls += 1
         return off
 
+    def _init_locs(self, loc_distribution, depot_distribution, params: dict, with_depot: bool):
+        """Resolve rl4co's `loc_distribution` / `depot_distribution` (envs/common/utils.py get_sampler) into
+        co_generate_locs laws.  Uniform keeps the generator's original streams; every other law needs the device."""
+        for key in ("loc_sampler", "depot_sampler"):
+            if params.get(key) is not None:
+                raise NotImplementedError(f"{key}: sampler objects are not supported; pass a distribution name")
+        self.loc_law = _location_law("loc", loc_distribution, self.min_loc, self.max_loc, params)
+        # a TSP instance has no depot; like rl4co's TSPGenerator, depot_distribution does not apply to it
+        self.depot_law = None
+        if with_depot and depot_distribution is not None:
+            self.depot_law = _location_law("depot", depot_distribution, self.min_loc, self.max_loc, params, depot=True)
+        laws = [law for law in (self.loc_law, self.depot_law) if law is not None]
+        if not self.on_device and any(kind != "uniform" for kind, _ in laws):
+            bad = loc_distribution if self.loc_law[0] != "uniform" else depot_distribution
+            raise NotImplementedError(f"location distribution {bad!r} is generated on the GPU only: pass "
+                                      "generator_params=dict(..., device=\"cuda\")")
+
+    def _draw_locs(self, law, shape, off: int, slot: int) -> torch.Tensor:
+        kind, kw = law
+        if not self.on_device:  # only uniform gets here (checked in _init_locs): the reference's torch call
+            return torch.rand(*shape) * (kw["hi"] - kw["lo"]) + kw["lo"]
+        if kind == "uniform" and slot == 0:  # the generator's original location stream
+            return native.generate_uniform(shape, self.device, self.seed, off, kw["lo"], kw["hi"])
+        return native.generate_locs(shape, self.device, self.seed, slot + off, kind, **kw)
+
+    def _sample_locs(self, batch_size, off: int, with_depot: bool):
+        """(depot [*B, 2] or None, locs [*B, num_loc, 2]) in the reference's order: without a depot law the depot is
+        node 0 of a (num_loc + 1)-node draw, otherwise the depot is drawn first and on its own."""
+        n = self.num_loc
+        loc_slot = 0 if self.loc_law[0] == "uniform" else _LOCS_SLOT
+        if self.depot_law is None:
+            locs = self._draw_locs(self.loc_law, (*batch_size, n + int(with_depot), 2), off, loc_slot)
+            return (locs[..., 0, :], locs[..., 1:, :]) if with_depot else (None, locs)
+        depot = self._draw_locs(self.depot_law, (*batch_size, 1, 2), off, _DEPOT_SLOT)[..., 0, :]
+        return depot, self._draw_locs(self.loc_law, (*batch_size, n, 2), off, loc_slot)
+
+
+# Offsets of the co_generate_locs streams.  The uniform streams of a generator use offsets calls * k with k <= 4, so
+# these ranges are never reached by them: adding a non-uniform law leaves every uniform draw as it was.
+_LOCS_SLOT, _DEPOT_SLOT = 1 << 62, 1 << 63
+
+#: parameters of the location laws (rl4co's get_sampler kwargs), accepted by every generator below
+LOC_PARAMS = ("n_cluster", "n_cluster_mix", "num_modes", "cdist", "loc_mean", "loc_std", "depot_mean", "depot_std")
+
+
+def _location_law(val_name: str, distribution, lo: float, hi: float, params: dict, depot: bool = False):
+    """rl4co/envs/common/utils.py get_sampler for locations -> (co_generate_locs kind, its keyword arguments)."""
+    from torch.distributions import Uniform
+
+    def need(*keys):
+        for k in keys:
+            if params.get(k) is None:
+                raise ValueError(f"{val_name}_distribution={distribution!r} needs the parameter {k!r}")
+        return [params[k] for k in keys]
+
+    if isinstance(distribution, (int, float)) and not isinstance(distribution, bool):
+        law = ("constant", dict(value=float(distribution)))
+    elif distribution is Uniform or distribution == "uniform":
+        law = ("uniform", dict(lo=float(lo), hi=float(hi)))
+    elif distribution in ("normal", "gaussian"):
+        mean, std = need(f"{val_name}_mean", f"{val_name}_std")
+        law = ("normal", dict(mean=float(mean), std=float(std)))
+    elif distribution == "center":  # the reference's formula: (max - min) / 2, the midpoint only when min = 0
+        law = ("constant", dict(value=(hi - lo) / 2))
+    elif distribution == "corner":
+        law = ("constant", dict(value=float(lo)))
+    elif not isinstance(distribution, str) or distribution in ("exponential", "poisson"):
+        raise NotImplementedError(f"{val_name}_distribution={distribution!r} is not supported: use a number, "
+                                  "'uniform', 'normal', 'center', 'corner', 'cluster', 'mixed', 'gaussian_mixture', "
+                                  "'mix_distribution' or 'mix_multi_distributions'")
+    elif depot and distribution in ("cluster", "mixed", "gaussian_mixture", "mix_distribution",
+                                    "mix_multi_distributions"):
+        raise ValueError(f"depot_distribution={distribution!r}: a single depot can only be drawn from a number, "
+                         "'uniform', 'normal', 'center' or 'corner'")
+    elif distribution == "cluster":
+        law = ("cluster", dict(n_cluster=int(need("n_cluster")[0])))
+    elif distribution == "mixed":
+        law = ("mixed", dict(n_cluster_mix=int(need("n_cluster_mix")[0])))
+    elif distribution == "gaussian_mixture":
+        m, c = need("num_modes", "cdist")
+        law = ("gaussian_mixture", dict(num_modes=int(m), cdist=float(c)))
+    elif distribution == "mix_distribution":
+        k, k_mix = need("n_cluster", "n_cluster_mix")
+        law = ("mix_distribution", dict(n_cluster=int(k), n_cluster_mix=int(k_mix)))
+    elif distribution == "mix_multi_distributions":
+        law = ("mix_multi_distributions", {})
+    else:
+        raise ValueError(f"Invalid distribution type of {distribution}")
+    return law
+
 
 class TSPGenerator(Generator, _DeviceStream):
-    """rl4co/envs/routing/tsp/generator.py:14-58 (uniform locations)."""
+    """rl4co/envs/routing/tsp/generator.py:14-58.  Locations follow `loc_distribution` (default uniform; see
+    `_location_law` for the others, which need `device="cuda"`)."""
 
-    def __init__(self, num_loc: int = 20, min_loc: float = 0.0, max_loc: float = 1.0, device=None, seed=None, **_):
+    def __init__(self, num_loc: int = 20, min_loc: float = 0.0, max_loc: float = 1.0, device=None, seed=None, *,
+                 loc_distribution="uniform", depot_distribution=None, **kwargs):
         self.num_loc, self.min_loc, self.max_loc = num_loc, min_loc, max_loc
         self._init_stream(device, seed)
+        self._init_locs(loc_distribution, depot_distribution, kwargs, with_depot=False)
 
     def _generate(self, batch_size) -> TensorDict:
+        _, locs = self._sample_locs(batch_size, self._next_offset(1) if self.on_device else 0, with_depot=False)
         if self.on_device:
-            locs = native.generate_uniform((*batch_size, self.num_loc, 2), self.device, self.seed, self._next_offset(1),
-                                           self.min_loc, self.max_loc)
             return TensorDict({"locs": locs}, batch_size=batch_size, device=self.device)
-        locs = torch.rand(*batch_size, self.num_loc, 2) * (self.max_loc - self.min_loc) + self.min_loc
         return TensorDict({"locs": locs}, batch_size=batch_size)
 
 
 class CVRPGenerator(Generator, _DeviceStream):
-    """rl4co/envs/routing/cvrp/generator.py:33-140 (uniform locations, integer demands 1..9
-    over the Kool et al. capacity table, depot = first sampled point)."""
+    """rl4co/envs/routing/cvrp/generator.py:33-140 (integer demands 1..9 over the Kool et al. capacity table).  Locations
+    follow `loc_distribution` (default uniform); the depot is the first sampled point unless `depot_distribution`
+    is given, in which case it is drawn on its own (see `_DeviceStream._init_locs`)."""
 
     def __init__(self, num_loc: int = 20, min_loc: float = 0.0, max_loc: float = 1.0, min_demand: int = 1,
                  max_demand: int = 10, vehicle_capacity: float = 1.0, capacity: float | None = None, device=None,
-                 seed=None, **_):
+                 seed=None, *, loc_distribution="uniform", depot_distribution=None, **kwargs):
         self._init_stream(device, seed)
         self.num_loc, self.min_loc, self.max_loc = num_loc, min_loc, max_loc
+        self._init_locs(loc_distribution, depot_distribution, kwargs, with_depot=True)
         self.min_demand, self.max_demand = min_demand, max_demand
         self.vehicle_capacity = vehicle_capacity
         if capacity is None:
@@ -91,20 +185,19 @@ class CVRPGenerator(Generator, _DeviceStream):
     def _generate(self, batch_size) -> TensorDict:
         if self.on_device:
             off = self._next_offset(2)
-            locs = native.generate_uniform((*batch_size, self.num_loc + 1, 2), self.device, self.seed, off,
-                                           self.min_loc, self.max_loc)
+            depot, locs = self._sample_locs(batch_size, off, with_depot=True)
             demand = native.generate_demand((*batch_size, self.num_loc), self.device, self.seed, off + 1,
                                             self.min_demand, self.max_demand, self.capacity)
             return TensorDict(
-                {"locs": locs[..., 1:, :], "depot": locs[..., 0, :], "demand": demand,
+                {"locs": locs, "depot": depot, "demand": demand,
                  "capacity": torch.full((*batch_size, 1), self.capacity, device=self.device)},
                 batch_size=batch_size, device=self.device)
-        locs = torch.rand(*batch_size, self.num_loc + 1, 2) * (self.max_loc - self.min_loc) + self.min_loc
+        depot, locs = self._sample_locs(batch_size, 0, with_depot=True)
         lo, hi = self.min_demand - 1, self.max_demand - 1
         demand = torch.rand(*batch_size, self.num_loc) * (hi - lo) + lo
         demand = (demand.int() + 1).float()
         return TensorDict(
-            {"locs": locs[..., 1:, :], "depot": locs[..., 0, :], "demand": demand / self.capacity,
+            {"locs": locs, "depot": depot, "demand": demand / self.capacity,
              "capacity": torch.full((*batch_size, 1), self.capacity)},
             batch_size=batch_size,
         )
@@ -114,14 +207,16 @@ OP_MAX_LENGTHS = {20: 2.0, 50: 3.0, 100: 4.0}  # rl4co/envs/routing/op/generator
 
 
 class OPGenerator(Generator, _DeviceStream):
-    """rl4co/envs/routing/op/generator.py:19-139: uniform locations (depot = first sampled point); prize by type --
+    """rl4co/envs/routing/op/generator.py:19-139: locations and depot as in CVRPGenerator; prize by type --
     "dist" (default, Fischetti et al. / Kool et al.: from the distance to the depot), "unif", "const"; max_length from
     the size table.  `device="cuda"`: locations from co_generate_uniform, prizes derived on the device."""
 
     def __init__(self, num_loc: int = 20, min_loc: float = 0.0, max_loc: float = 1.0, prize_type: str = "dist",
-                 max_length: float | None = None, device=None, seed=None, **_):
+                 max_length: float | None = None, device=None, seed=None, *, loc_distribution="uniform",
+                 depot_distribution=None, **kwargs):
         self._init_stream(device, seed)
         self.num_loc, self.min_loc, self.max_loc = num_loc, min_loc, max_loc
+        self._init_locs(loc_distribution, depot_distribution, kwargs, with_depot=True)
         if prize_type not in ("dist", "unif", "const"):
             raise ValueError(f"Invalid prize_type: {prize_type}")
         self.prize_type = prize_type
@@ -131,35 +226,33 @@ class OPGenerator(Generator, _DeviceStream):
 
     def _generate(self, batch_size) -> TensorDict:
         dev = self.device if self.on_device else None
-        if self.on_device:
-            locs = native.generate_uniform((*batch_size, self.num_loc + 1, 2), self.device, self.seed,
-                                           self._next_offset(2), self.min_loc, self.max_loc)
-        else:
-            locs = torch.rand(*batch_size, self.num_loc + 1, 2) * (self.max_loc - self.min_loc) + self.min_loc
+        depot, locs = self._sample_locs(batch_size, self._next_offset(2) if self.on_device else 0, with_depot=True)
         if self.prize_type == "const":
             prize = torch.ones(*batch_size, self.num_loc, device=dev)
         elif self.prize_type == "unif":
             prize = (1 + torch.randint(0, 100, (*batch_size, self.num_loc), device=dev).float()) / 100
         else:
-            prize = (locs[..., 0:1, :] - locs[..., 1:, :]).norm(p=2, dim=-1)
+            prize = (depot[..., None, :] - locs).norm(p=2, dim=-1)
             prize = (1 + (prize / prize.max(dim=-1, keepdim=True)[0] * 99).int()).float() / 100
         if isinstance(self.max_length, torch.Tensor):
             max_length = self.max_length
         else:
             max_length = torch.full((*batch_size,), self.max_length, device=dev)
-        return TensorDict({"locs": locs[..., 1:, :], "depot": locs[..., 0, :], "prize": prize, "max_length": max_length},
+        return TensorDict({"locs": locs, "depot": depot, "prize": prize, "max_length": max_length},
                           batch_size=batch_size, device=dev)
 
 
 class PCTSPGenerator(Generator, _DeviceStream):
-    """rl4co/envs/routing/pctsp/generator.py:14-139: uniform locations (depot = first sampled point), penalties
+    """rl4co/envs/routing/pctsp/generator.py:14-139: locations and depot as in CVRPGenerator, penalties
     U(0, max_penalty * penalty_factor / num_loc), deterministic prizes U(0, 4 / num_loc), stochastic prizes U(0, 2) x
     deterministic -- sampled in that order.  `device="cuda"`: Philox streams of co_generate_uniform."""
 
     def __init__(self, num_loc: int = 20, min_loc: float = 0.0, max_loc: float = 1.0, penalty_factor: float = 3.0,
-                 prize_required: float = 1.0, max_penalty: float | None = None, device=None, seed=None, **_):
+                 prize_required: float = 1.0, max_penalty: float | None = None, device=None, seed=None, *,
+                 loc_distribution="uniform", depot_distribution=None, **kwargs):
         self._init_stream(device, seed)
         self.num_loc, self.min_loc, self.max_loc = num_loc, min_loc, max_loc
+        self._init_locs(loc_distribution, depot_distribution, kwargs, with_depot=True)
         self.prize_required = prize_required
         if max_penalty is None:
             max_penalty = OP_MAX_LENGTHS.get(num_loc) or OP_MAX_LENGTHS[min(OP_MAX_LENGTHS, key=lambda x: abs(x - num_loc))]
@@ -170,16 +263,16 @@ class PCTSPGenerator(Generator, _DeviceStream):
         if self.on_device:
             off = self._next_offset(4)
             u = lambda shape, k, hi: native.generate_uniform(shape, self.device, self.seed, off + k, 0.0, hi)  # noqa: E731
-            locs = native.generate_uniform((*batch_size, n + 1, 2), self.device, self.seed, off, self.min_loc, self.max_loc)
+            depot, locs = self._sample_locs(batch_size, off, with_depot=True)
             penalty, det, sto = u((*batch_size, n), 1, self.max_penalty), u((*batch_size, n), 2, 4.0 / n), u((*batch_size, n), 3, 2.0)
             dev = self.device
         else:
-            locs = torch.rand(*batch_size, n + 1, 2) * (self.max_loc - self.min_loc) + self.min_loc
+            depot, locs = self._sample_locs(batch_size, 0, with_depot=True)
             penalty = torch.rand(*batch_size, n) * self.max_penalty
             det = torch.rand(*batch_size, n) * (4.0 / n)
             sto = torch.rand(*batch_size, n) * 2.0
             dev = None
-        return TensorDict({"locs": locs[..., 1:, :], "depot": locs[..., 0, :], "penalty": penalty, "deterministic_prize": det,
+        return TensorDict({"locs": locs, "depot": depot, "penalty": penalty, "deterministic_prize": det,
                            "stochastic_prize": sto * det}, batch_size=batch_size, device=dev)
 
 

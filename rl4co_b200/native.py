@@ -42,7 +42,7 @@ EXPORTS = [
     "co_cache_width", "co_rollout_max_nodes", "co_rollout", "co_reward_stats", "co_split_tf32", "co_gemm_tf32x3", "co_encoder_mha",
     "co_ffn_fused", "co_ffn_tile_weights", "co_ffn_tiled_weight_floats", "co_generate_uniform", "co_generate_demand", "co_dihedral8",
     "co_sdvrp_step", "co_sdvrp_action_mask", "co_attn_fwd", "co_attn_bwd", "co_instance_norm", "co_op_step", "co_op_action_mask", "co_op_reward", "co_pctsp_step", "co_pctsp_action_mask",
-    "co_tsp_two_opt",
+    "co_tsp_two_opt", "co_generate_locs",
 ]
 
 
@@ -76,6 +76,18 @@ class AttnArgs(Structure):
                 + [(n, ctypes.c_int64) for n in ("q_bs", "k_bs", "v_bs", "o_bs", "dq_bs", "dk_bs", "dv_bs")]
                 + [(n, c_int32) for n in ("q_rs", "k_rs", "v_rs", "o_rs", "dq_rs", "dk_rs", "dv_rs")]
                 + [("scale", c_float)])
+
+
+class LocsArgs(Structure):
+    _fields_ = [("B", ctypes.c_int64), ("N", c_int32), ("kind", c_int32), ("seed", c_uint64), ("offset", c_uint64),
+                ("lo", c_float), ("hi", c_float), ("mean", c_float), ("std", c_float), ("n_cluster", c_int32),
+                ("n_cluster_mix", c_int32), ("num_modes", c_int32), ("cdist", c_float)]
+
+
+#: co_generate_locs kinds (CO_LOCS_* in corollout.h)
+LOCS_KIND = {"uniform": 0, "constant": 1, "normal": 2, "cluster": 3, "mixed": 4, "gaussian_mixture": 5,
+             "mix_distribution": 6, "mix_multi_distributions": 7}
+LOCS_MAX_NODES = 10000
 
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -164,6 +176,7 @@ def lib() -> ctypes.CDLL:
     L.co_generate_uniform.argtypes = [c_void_p, ctypes.c_long, c_uint64, c_uint64, c_float, c_float, c_void_p]
     L.co_generate_demand.argtypes = [c_void_p, ctypes.c_long, c_uint64, c_uint64, c_int, c_int, c_float, c_void_p]
     L.co_dihedral8.argtypes = [c_void_p, c_void_p, ctypes.c_long, c_int, c_void_p]
+    L.co_generate_locs.argtypes = [c_void_p, POINTER(LocsArgs), c_void_p]
     _lib = L
     return L
 
@@ -505,6 +518,32 @@ def generate_demand(shape, device, seed: int, offset: int, min_demand: int, max_
     with torch.cuda.device(out.device):
         _check(lib().co_generate_demand(_ptr(out, F32, "out"), out.numel(), int(seed), int(offset), int(min_demand),
                                         int(max_demand), float(capacity), _stream()), "co_generate_demand")
+    return out
+
+
+def generate_locs(shape, device, seed: int, offset: int, kind: str, *, lo: float = 0.0, hi: float = 1.0,
+                  value: float = 0.0, mean: float = 0.0, std: float = 1.0, n_cluster: int = 0, n_cluster_mix: int = 0,
+                  num_modes: int = 0, cdist: float = 0.0):
+    """co_generate_locs: float32 locations of shape (*batch, N, 2) from one law (`kind` in LOCS_KIND; see corollout.h)
+    generated on the device.  "uniform" uses lo / hi, "constant" value, "normal" mean / std, "cluster" n_cluster,
+    "mixed" n_cluster_mix, "mix_distribution" both, "gaussian_mixture" num_modes / cdist."""
+    if kind not in LOCS_KIND:
+        raise ValueError(f"generate_locs: unknown kind {kind!r} (one of {sorted(LOCS_KIND)})")
+    shape = tuple(int(d) for d in shape)
+    if len(shape) < 2 or shape[-1] != 2:
+        raise ValueError(f"generate_locs: expected a shape (*batch, N, 2), got {shape}")
+    if torch.device(device).type != "cuda":
+        raise NativeLibraryError(f"generate_locs: libcorollout generates on CUDA devices (got {device}); "
+                                 "there is no CPU fallback")
+    out = torch.empty(shape, dtype=F32, device=device)
+    a = LocsArgs()
+    a.B, a.N, a.kind = out.numel() // max(1, 2 * shape[-2]), shape[-2], LOCS_KIND[kind]
+    a.seed, a.offset = int(seed), int(offset)
+    a.lo, a.hi = (float(value), float(value)) if kind == "constant" else (float(lo), float(hi))
+    a.mean, a.std = float(mean), float(std)
+    a.n_cluster, a.n_cluster_mix, a.num_modes, a.cdist = int(n_cluster), int(n_cluster_mix), int(num_modes), float(cdist)
+    with torch.cuda.device(out.device):
+        _check(lib().co_generate_locs(_ptr(out, F32, "out"), ctypes.byref(a), _stream()), "co_generate_locs")
     return out
 
 

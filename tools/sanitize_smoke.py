@@ -70,3 +70,13 @@ for n in (20, 224, 300):
     native.tsp_two_opt(tours, 50, distances=d, iterations=its)
 torch.cuda.synchronize()
 print("local search ok")
+# location laws (co_generate_locs): every kind, including the shared-memory shuffle (mixed) and the counting sort by
+# mode (gaussian_mixture), at sizes on both sides of a full CTA and at the node limit
+for n in (2, 33, 300, 10000):
+    for kind, kw in (("uniform", {}), ("constant", dict(value=0.5)), ("normal", dict(mean=0.5, std=0.1)),
+                     ("cluster", dict(n_cluster=3)), ("mixed", dict(n_cluster_mix=2)),
+                     ("gaussian_mixture", dict(num_modes=1, cdist=1)), ("gaussian_mixture", dict(num_modes=5, cdist=30)),
+                     ("mix_distribution", dict(n_cluster=3, n_cluster_mix=1)), ("mix_multi_distributions", {})):
+        native.generate_locs((5, n, 2), dev, 1, 0, kind, **kw)
+torch.cuda.synchronize()
+print("generate_locs ok")
