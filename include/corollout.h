@@ -304,6 +304,16 @@ int co_generate_demand(float* out, long n, uint64_t seed, uint64_t offset, int m
                        float capacity, void* stream);
 int co_dihedral8(const float* locs, float* out, long B, int N, void* stream);
 
+/* co_symmetric_augment: base [B, N, 2], phi [S*B] (one angle per augmented row, drawn by the caller) ->
+ * out [S*B, N, 2], aug-major (row a*B + b is image a of instance b).  Per node, as symmetric_transform
+ * (data/transforms.py:49-69):  x0 = x - 0.5, y0 = y - 0.5;  x' = cos(phi) x0 - sin(phi) y0,
+ * y' = sin(phi) x0 + cos(phi) y0;  (x', y') swapped when phi > 2*pi (2*pi rounded to fp32);  + 0.5.
+ * Every operation is rounded on its own (no FMA) and cos / sin are the precise ones, so the result equals torch's
+ * elementwise kernels bit for bit; rows with phi = 0 are (x - 0.5) + 0.5, not copies.  The reference draws
+ * phi = U[0, 1) * 4 * pi with phi[:B] = 0 (transforms.py:80-84).  Null pointers, B < 0, S < 1, N < 1 or a
+ * base / out that is not 8-byte aligned are CO_ERR_BAD_ARG. */
+int co_symmetric_augment(const float* base, const float* phi, float* out, long B, int S, int N, void* stream);
+
 /* co_generate_locs: out [B, N, 2] float32 locations from one location law (envs/common/utils.py get_sampler and
  * envs/common/distribution_utils.py), one CTA per instance.  Philox4x32-10 keyed by `seed` with the counter
  * (instance, draw index, offset): row b is the same for every B > b, launch shape and GPU.

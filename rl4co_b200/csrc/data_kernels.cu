@@ -6,6 +6,8 @@
 //   co_generate_demand    <- rl4co/envs/routing/cvrp/generator.py:126-137: (floor(U[lo,hi)) + 1) / capacity with
 //                            lo = min_demand - 1, hi = max_demand - 1
 //   co_dihedral8          <- rl4co/data/transforms.py:16-38 (aug-major: row a*B + b)
+//   co_symmetric_augment  <- rl4co/data/transforms.py:49-86 (rotation about (0.5, 0.5), reflection for phi > 2*pi;
+//                            aug-major; the angles come from the caller)
 // The random stream is Philox4x32-10 keyed by (seed, offset): same seed -> same instances on every run and on every
 // GPU; it is NOT torch's CPU stream, so generated instances are distributionally, not bit-wise, the reference's.
 #include "co_common.cuh"
@@ -64,6 +66,54 @@ __global__ void __launch_bounds__(256) dihedral8_kernel(const float2* __restrict
     out[5 * BN + i] = make_float2(ry, x);
     out[6 * BN + i] = make_float2(y, rx);
     out[7 * BN + i] = make_float2(ry, rx);
+  }
+}
+
+// symmetric_transform (transforms.py:49-69) with torch's rounding: every operation is its own elementwise kernel in
+// the reference, so each is rounded on its own here (__f*_rn: no FMA contraction) and cos / sin are the precise
+// cosf / sinf.  The reflection test compares against 2*pi rounded to fp32, as torch does for an fp32 tensor.
+constexpr float TWO_PI_F32 = 6.28318530717958647692f;
+
+// One warp per 32 consecutive nodes of the flattened base [B*N]: each lane reads its node once and writes its S
+// images.  The warp's nodes belong to nw <= 32 consecutive instances, so one cos / sin evaluation by the whole warp
+// covers 32 / nw images of all of them: lane l takes instance b0 + l % nw of image a0 + l / nw, and each lane fetches
+// its own (image, instance) values with shuffles.  Every loop bound is warp-uniform.
+__global__ void __launch_bounds__(256) symmetric_augment_kernel(const float2* __restrict__ xy,
+                                                                const float* __restrict__ phi,
+                                                                float2* __restrict__ out, long B, int S, int N) {
+  const long BN = B * (long)N;
+  const int lane = threadIdx.x & 31;
+  const long nwarps = (long)gridDim.x * (blockDim.x >> 5);
+  for (long w = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w * 32 < BN; w += nwarps) {
+    const long i0 = w * 32, i = i0 + lane, b0 = i0 / N;
+    const bool live = i < BN;
+    const int k = (int)(i0 - b0 * N + lane) / N;                    // this lane's instance is b0 + k
+    const int nw = (int)((i0 + 31 < BN ? i0 + 31 : BN - 1) / N - b0) + 1;  // instances in this warp
+    const int per = 32 / nw;                                            // images per cos / sin evaluation
+    const long pb = b0 + lane % nw;
+    float x0 = 0.f, y0 = 0.f;
+    if (live) {
+      const float2 p = xy[i];
+      x0 = __fsub_rn(p.x, 0.5f);
+      y0 = __fsub_rn(p.y, 0.5f);
+    }
+    for (int a0 = 0; a0 < S; a0 += per) {
+      const int pa = a0 + lane / nw;
+      const float f = pa < S && lane < per * nw ? phi[(long)pa * B + pb] : 0.f;
+      const float cf = cosf(f), sf = sinf(f);
+      const int na = S - a0 < per ? S - a0 : per;
+      for (int j = 0; j < na; ++j) {
+        const int src = j * nw + k;
+        const float c = __shfl_sync(FULL, cf, src), s = __shfl_sync(FULL, sf, src);
+        const bool reflect = __shfl_sync(FULL, f, src) > TWO_PI_F32;
+        if (live) {
+          const float xr = __fsub_rn(__fmul_rn(c, x0), __fmul_rn(s, y0));
+          const float yr = __fadd_rn(__fmul_rn(s, x0), __fmul_rn(c, y0));
+          out[(long)(a0 + j) * BN + i] = reflect ? make_float2(__fadd_rn(yr, 0.5f), __fadd_rn(xr, 0.5f))
+                                                 : make_float2(__fadd_rn(xr, 0.5f), __fadd_rn(yr, 0.5f));
+        }
+      }
+    }
   }
 }
 
@@ -316,6 +366,17 @@ extern "C" int co_dihedral8(const float* locs, float* out, long B, int N, void* 
   if (B == 0) return CO_OK;
   dihedral8_kernel<<<stream_grid(B * N), 256, 0, (cudaStream_t)stream>>>((const float2*)locs, (float2*)out, B * (long)N);
   return check_launch("co_dihedral8");
+}
+
+extern "C" int co_symmetric_augment(const float* base, const float* phi, float* out, long B, int S, int N,
+                                    void* stream) {
+  if (!base || !phi || !out) return fail(CO_ERR_BAD_ARG, "co_symmetric_augment: null pointer%s");
+  if (B < 0 || S < 1 || N < 1) return fail(CO_ERR_BAD_ARG, "co_symmetric_augment: bad shape%s");
+  if (((uintptr_t)base | (uintptr_t)out) & 7) return fail(CO_ERR_BAD_ARG, "co_symmetric_augment: base / out must be 8-byte aligned%s");
+  if (B == 0) return CO_OK;
+  symmetric_augment_kernel<<<stream_grid(B * N), 256, 0, (cudaStream_t)stream>>>(
+      (const float2*)base, phi, (float2*)out, B, S, N);
+  return check_launch("co_symmetric_augment");
 }
 
 extern "C" int co_generate_locs(float* out, const co_locs_args* args, void* stream) {

@@ -42,7 +42,7 @@ EXPORTS = [
     "co_cache_width", "co_rollout_max_nodes", "co_rollout", "co_reward_stats", "co_split_tf32", "co_gemm_tf32x3", "co_encoder_mha",
     "co_ffn_fused", "co_ffn_tile_weights", "co_ffn_tiled_weight_floats", "co_generate_uniform", "co_generate_demand", "co_dihedral8",
     "co_sdvrp_step", "co_sdvrp_action_mask", "co_attn_fwd", "co_attn_bwd", "co_instance_norm", "co_op_step", "co_op_action_mask", "co_op_reward", "co_pctsp_step", "co_pctsp_action_mask",
-    "co_tsp_two_opt", "co_generate_locs",
+    "co_tsp_two_opt", "co_generate_locs", "co_symmetric_augment",
 ]
 
 
@@ -176,6 +176,7 @@ def lib() -> ctypes.CDLL:
     L.co_generate_uniform.argtypes = [c_void_p, ctypes.c_long, c_uint64, c_uint64, c_float, c_float, c_void_p]
     L.co_generate_demand.argtypes = [c_void_p, ctypes.c_long, c_uint64, c_uint64, c_int, c_int, c_float, c_void_p]
     L.co_dihedral8.argtypes = [c_void_p, c_void_p, ctypes.c_long, c_int, c_void_p]
+    L.co_symmetric_augment.argtypes = [c_void_p, c_void_p, c_void_p, ctypes.c_long, c_int, c_int, c_void_p]
     L.co_generate_locs.argtypes = [c_void_p, POINTER(LocsArgs), c_void_p]
     _lib = L
     return L
@@ -553,6 +554,21 @@ def dihedral8(locs):
     B, N, _ = locs.shape
     out = torch.empty(8 * B, N, 2, dtype=F32, device=locs.device)
     _check(lib().co_dihedral8(_ptr(locs, F32, "locs"), _ptr(out, F32, "out"), B, N, _stream()), "co_dihedral8")
+    return out
+
+
+@_on_device_of_first_tensor
+def symmetric_augment(base, phi, S: int):
+    """[B, N, 2] + angles [S*B] -> [S*B, N, 2] (aug-major): row a*B + b is instance b rotated by phi[a*B + b] about
+    (0.5, 0.5) and reflected when that angle exceeds 2*pi (rl4co/data/transforms.py:49-69), one kernel."""
+    if base.dim() != 3 or base.shape[-1] != 2:
+        raise ValueError(f"base: expected [B, N, 2], got {tuple(base.shape)}")
+    B, N, _ = base.shape
+    if S < 1 or tuple(phi.shape) != (S * B,):
+        raise ValueError(f"phi: expected [{S} * {B}] angles, got {tuple(phi.shape)}")
+    out = torch.empty(S * B, N, 2, dtype=F32, device=base.device)
+    _check(lib().co_symmetric_augment(_ptr(base, F32, "base"), _ptr(phi, F32, "phi"), _ptr(out, F32, "out"), B, int(S),
+                                      N, _stream()), "co_symmetric_augment")
     return out
 
 

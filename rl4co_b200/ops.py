@@ -7,6 +7,8 @@ views and index arithmetic in torch on whatever device the data lives; the arith
 
 from __future__ import annotations
 
+import math
+
 import torch
 
 from .tensordict import TensorDict
@@ -92,23 +94,94 @@ def dihedral_8_augmentation(xy):
     return torch.cat([torch.cat(z, dim=2) for z in zs], dim=0)
 
 
-class StateAugmentation:
-    """rl4co/data/transforms.py:113-151 restricted to the dihedral-8 function POMO uses."""
+def symmetric_transform(x, y, phi, offset: float = 0.5):
+    """rl4co/data/transforms.py:49-69: rotation by phi about (offset, offset), then x <-> y where phi > 2*pi."""
+    x, y = x - offset, y - offset
+    x_prime = torch.cos(phi) * x - torch.sin(phi) * y
+    y_prime = torch.sin(phi) * x + torch.cos(phi) * y
+    mask = phi > 2 * math.pi
+    xy = torch.cat((x_prime, y_prime), dim=-1)
+    xy = torch.where(mask, xy.flip(-1), xy)
+    return xy + offset
 
-    def __init__(self, num_augment: int = 8, augment_fn: str = "dihedral8", feats=None, **_):
-        assert augment_fn == "dihedral8" and num_augment == 8, "only dihedral8 x8 is on the hot path"
+
+def symmetric_angles(xy, num_augment: int, first_augment: bool = False):
+    """rl4co/data/transforms.py:80-84: one angle in [0, 4*pi) per row of the batchified xy (torch's stream, same
+    expression and call order), 0 for the first 1/num_augment rows unless first_augment."""
+    phi = torch.rand(xy.shape[0], device=xy.device) * 4 * math.pi
+    if not first_augment:
+        phi[: xy.shape[0] // num_augment] = 0.0
+    return phi
+
+
+def symmetric_augmentation(xy, num_augment: int = 8, first_augment: bool = False):
+    """rl4co/data/transforms.py:72-86 (aug-major: flat index = a * B + b)."""
+    phi = symmetric_angles(xy, num_augment, first_augment)
+    x, y = xy[..., [0]], xy[..., [1]]
+    return symmetric_transform(x, y, phi[:, None, None])
+
+
+def min_max_normalize(x):
+    """rl4co/data/transforms.py:89-90: one min / max over the whole tensor."""
+    return (x - x.min()) / (x.max() - x.min())
+
+
+class StateAugmentation:
+    """rl4co/data/transforms.py:105-151.
+
+    `augment_fn` is "dihedral8" (num_augment must be 8), "symmetric" (a random rotation about (0.5, 0.5), reflected
+    half of the time, any num_augment) or a callable fn(batchified feature, num_augment).  The default stays
+    "dihedral8" (rl4co's is "symmetric"), so that existing callers keep the dihedral-8 augmentation POMO uses.
+    On a CUDA fp32 [B, N, 2] feature both named laws run as one kernel from the un-batchified rows; elsewhere they
+    run the reference's torch expressions.  The angles of "symmetric" are drawn from torch's generator as the
+    reference draws them, so a seed gives the reference's tensors bit for bit on either device."""
+
+    def __init__(self, num_augment: int = 8, augment_fn="dihedral8", first_aug_identity: bool = True,
+                 normalize: bool = False, feats=None, **_):
+        if not callable(augment_fn) and augment_fn not in ("dihedral8", "symmetric"):
+            raise ValueError(f"Unknown augment_fn: {augment_fn}. Available options: 'symmetric', 'dihedral8' or a "
+                             "custom callable")
+        assert not (augment_fn == "dihedral8" and num_augment != 8), (
+            "When using the `dihedral8` augmentation function, then num_augment must be 8")
         self.num_augment = num_augment
+        self.augment_fn = augment_fn
+        self.first_aug_identity = first_aug_identity
+        self.normalize = normalize
         self.feats = ["locs"] if feats is None else feats
+
+    def _augment(self, x, base):
+        """Augmented [S*B, ...] feature from the batchified x; `base` is its un-batchified [B, ...] source, or None
+        when x's rows are not S copies of it (a feature listed twice in feats)."""
+        S = self.num_augment
+        if callable(self.augment_fn):
+            return self.augment_fn(x, S)
+        if self.augment_fn == "dihedral8":
+            first = x[: x.shape[0] // 8]  # transforms.py:40-46 augments the first 1/8 of the rows
+            if first.is_cuda and first.dim() == 3 and first.shape[-1] == 2 and first.dtype == torch.float32:
+                from . import native
+
+                return native.dihedral8(first.contiguous())  # one kernel: 8 B read, 64 B written per node
+            return dihedral_8_augmentation(first)
+        if (base is not None and base.is_cuda and base.dim() == 3 and base.shape[-1] == 2
+                and base.dtype == torch.float32):
+            from . import native
+
+            return native.symmetric_augment(base.contiguous(), symmetric_angles(x, S), S)  # per node: 8 B read, 8 S B written
+        return symmetric_augmentation(x, S)
 
     def __call__(self, td: TensorDict) -> TensorDict:
         td_aug = batchify(td, self.num_augment)
+        done = set()
         for feat in self.feats:
-            x = td_aug[feat]
-            base = x[: x.shape[0] // 8]
-            if base.is_cuda and base.dim() == 3 and base.shape[-1] == 2 and base.dtype == torch.float32:
-                from . import native
-
-                td_aug.set(feat, native.dihedral8(base.contiguous()))  # one kernel: 8 B read, 64 B written per node
-            else:
-                td_aug.set(feat, dihedral_8_augmentation(base))
+            if not self.first_aug_identity:
+                # transforms.py:142,147 keep td_aug[feat][[B], 0], i.e. node 0 of row B (image 1 of instance 0), not
+                # augmentation 0 as the reference's docstring says; reproduced as the reference computes it
+                init_aug_feat = td_aug[feat][list(td.size()), 0].clone()
+            aug_feat = self._augment(td_aug[feat], None if feat in done else td[feat])
+            if self.normalize:
+                aug_feat = min_max_normalize(aug_feat)
+            if not self.first_aug_identity:
+                aug_feat[list(td.size()), 0] = init_aug_feat
+            td_aug.set(feat, aug_feat)
+            done.add(feat)
         return td_aug

@@ -2,7 +2,7 @@
 
   REINFORCE.shared_step / calculate_loss   rl4co/models/rl/reinforce/reinforce.py:59-111
   baselines (no / shared / mean / exponential / rollout)   rl4co/models/rl/reinforce/baselines.py:48-248
-  POMO.shared_step (dihedral-8 aug x multistart, max over starts / augs)   rl4co/models/zoo/pomo/model.py:88-143
+  POMO.shared_step (augmentation x multistart, max over starts / augs, best tours)   rl4co/models/zoo/pomo/model.py:88-143
   Evaluate decoding (teacher forcing)      rl4co/utils/decoding.py:448-461, constructive/base.py:202-203
 
 Training needs d(log-likelihood)/d(theta).  The fused rollout kernel is forward-only, so a
@@ -546,14 +546,18 @@ def reinforce_step(policy, env, td, baseline, optimizer=None, decode_type="sampl
     return res
 
 
-def pomo_step(policy, env, td, num_augment=8, num_starts=None, phase="test", optimizer=None):
-    """POMO.shared_step (pomo/model.py:88-143): optional dihedral-8 augmentation (val/test),
-    multistart rollout, shared baseline over starts; returns max rewards over starts / augs."""
+def pomo_step(policy, env, td, num_augment=8, num_starts=None, phase="test", optimizer=None, augment_fn="dihedral8",
+              first_aug_identity=True, feats=None):
+    """POMO.shared_step (pomo/model.py:88-143): optional augmentation (val/test; `augment_fn`, `first_aug_identity`
+    and `feats` as POMO passes them to StateAugmentation), multistart rollout, shared baseline over starts; returns
+    max rewards over starts / augs and, on val/test, the tours behind them: `best_multistart_actions` [B, aug, T]
+    ([B, T] without augmentation) and `best_aug_actions` [B, T]."""
     B = td.batch_size[0]
     n_aug = num_augment if phase != "train" else 0
     n_start = env.get_num_starts(td) if num_starts is None else num_starts
     if n_aug > 1:
-        td = StateAugmentation(num_augment=n_aug)(td)
+        td = StateAugmentation(num_augment=n_aug, augment_fn=augment_fn, first_aug_identity=first_aug_identity,
+                               feats=feats)(td)
     if phase == "train":
         policy.train()
         enc = policy.encoder(td)
@@ -574,8 +578,10 @@ def pomo_step(policy, env, td, num_augment=8, num_starts=None, phase="test", opt
         out = policy(td, env, phase=phase, decode_type="multistart_greedy", num_starts=n_start)
     shape = (n_aug, n_start) if n_aug > 1 else (n_start,)
     reward = unbatchify(out["reward"], shape)                               # [B, aug, start] | [B, start]
-    max_reward = reward.max(-1)[0]
-    res = {"reward": reward, "max_reward": max_reward, "actions": out["actions"]}
+    max_reward, max_idxs = reward.max(-1)
+    best_ms = gather_by_index(unbatchify(out["actions"], shape), max_idxs, dim=max_idxs.dim())  # [B, aug, T] | [B, T]
+    res = {"reward": reward, "max_reward": max_reward, "actions": out["actions"], "best_multistart_actions": best_ms}
     if n_aug > 1:
-        res["max_aug_reward"] = max_reward.max(1)[0]
+        res["max_aug_reward"], aug_idxs = max_reward.max(1)
+        res["best_aug_actions"] = gather_by_index(best_ms, aug_idxs)             # [B, T]
     return res

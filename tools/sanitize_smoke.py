@@ -80,3 +80,9 @@ for n in (2, 33, 300, 10000):
         native.generate_locs((5, n, 2), dev, 1, 0, kind, **kw)
 torch.cuda.synchronize()
 print("generate_locs ok")
+# symmetric augmentation (co_symmetric_augment): one node per instance (a warp spans 32 instances), warps straddling
+# instances, and a partial last warp
+for B, S, N in ((37, 3, 1), (5, 8, 20), (3, 2, 1000)):
+    native.symmetric_augment(torch.rand(B, N, 2, device=dev), torch.rand(S * B, device=dev) * 4 * torch.pi, S)
+torch.cuda.synchronize()
+print("symmetric_augment ok")
