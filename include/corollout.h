@@ -145,6 +145,47 @@ int co_check_tours(const int64_t* actions, const float* demand,
 int co_tsp_two_opt(const float* locs, const float* dist, const int64_t* tours_in, int64_t* tours_out,
                    int32_t* iterations, int B, int N, int max_iterations, void* stream);
 
+/* CVRPEnv.local_search  (rl4co/envs/routing/cvrp/env.py -> cvrp/local_search.py): the project's own deterministic
+ * local search behind the reference's signature and output layout.  It is not HGS-CVRP's SWAP*.
+ *   Inputs: N customers; tours_in [B,T] int64 in the action format (0 = depot; leading, trailing and repeated zeros
+ *   allowed); demand [B,N] (customers, already divided by the capacity); capacity [B]; exactly one of
+ *     locs [B,N+1,2]   -> d[a,b] = sqrt(fma(dy, dy, dx*dx)), dx = x_a - x_b (get_distance_matrix on the CPU), or
+ *     dist [B,N+1,N+1] -> used as given (possibly asymmetric); the diagonal is read as given (d[0][0] = 0 from locs).
+ *   Routes: the maximal runs of customers of the tour, numbered in input order (slot r); each keeps its slot, a start
+ *   depot with id N+1+r and an end depot, also when a move empties it (it may be refilled; no route is added).  A
+ *   depot id reads row / column 0.  p(x) / s(x) are the predecessor / successor within the route.  The load of a route
+ *   is the fp32 left-to-right sum of its demands in route order, recomputed after every move for the routes it changed;
+ *   pre(x) is the load up to and including x (0 at a start depot).  lim = capacity + 1e-5f.
+ *   Search: best improvement.  A sweep scores every candidate below in fp32, each operation rounded on its own in the
+ *   order parenthesised, and takes the smallest key (delta, kind, u, v); the move is applied when delta < -1e-6 (as a
+ *   double).  Sweeps repeat until none improves or max_iterations moves have been applied (<= 0: no move).
+ *     kind 0 relocate  u customer, v customer or start depot, v not in {u, p(u)}: u moves after v.
+ *       delta = ((d[pu][su] - d[pu][u]) - d[u][su]) + ((d[v][u] + d[u][sv]) - d[v][sv])
+ *       admissible: same route: load <= lim; else load(u's) - dem[u] <= lim and load(v's) + dem[u] <= lim
+ *     kind 1 swap      customers u < v, su != v and sv != u: u and v exchange places.
+ *       delta = (((d[pu][v] + d[v][su]) - d[pu][u]) - d[u][su]) + (((d[pv][u] + d[u][sv]) - d[pv][v]) - d[v][sv])
+ *       admissible: same route: load <= lim; else (load(u's) - dem[u]) + dem[v] <= lim and
+ *       (load(v's) - dem[v]) + dem[u] <= lim
+ *     kind 2 2-opt     u (customer or start depot) before customer v in one route, su != v: su..v is reversed.
+ *       delta = ((d[u][v] + d[su][sv]) - d[u][su]) - d[v][sv]                  admissible: load <= lim
+ *     kind 3 2-opt*    u in route A, v in route B, A < B, not both start depots, su and sv not both end depots:
+ *       A becomes A[..u] + B[sv..], B becomes B[..v] + A[su..].
+ *       delta = ((d[u][sv] + d[v][su]) - d[u][su]) - d[v][sv]
+ *       admissible: pre(u) + (load(B) - pre(v)) <= lim and pre(v) + (load(A) - pre(u)) <= lim
+ *   Outputs: tours_out [B,2N] int64 as the reference's merge_subroutes without its leading column: the non-empty
+ *   routes in slot order, one 0 between routes, no leading 0, zero padding; used_len [B] int32 = entries before the
+ *   padding.  iterations [B] (nullable): moves applied.  feasible [B] (nullable): 1 when tours_out passes the capacity
+ *   rule of CVRPEnv.check_solution_validity (running load, a depot visit subtracts the capacity and clamps at 0, load
+ *   <= capacity + 1e-5 after every step), else 0.  A row holding an id outside [0, N], or that does not visit every
+ *   customer exactly once, is copied through (its first min(T, 2N) entries, then zeros) with used_len = min(T, 2N),
+ *   iterations = -1 and feasible = 0.  tours_out must not overlap tours_in.
+ *   Errors: a null pointer, both or neither of locs / dist, B < 0, N < 1, T < 1, or a pointer not aligned to its
+ *   element (8 bytes for locs) is CO_ERR_BAD_ARG; N + 1 > CO_TWO_OPT_MAX_NODES is CO_ERR_UNSUPPORTED.  The matrix is
+ *   held in shared memory up to N + 1 = CO_TWO_OPT_RESIDENT_MAX_NODES nodes; every path gives the same tours. */
+int co_cvrp_local_search(const float* locs, const float* dist, const float* demand, const float* capacity,
+                         const int64_t* tours_in, int64_t* tours_out, int32_t* used_len, int32_t* iterations,
+                         int32_t* feasible, int B, int N, int T, int max_iterations, void* stream);
+
 /* ------------------------------------------------------------------ decoder, one step */
 
 /* Weights of the decoder path, device pointers, all float32, no biases

@@ -546,6 +546,47 @@ class FusedCVRPEnv(FusedEnvBase):
         assert bad == 0, "Invalid tour"
 
     @staticmethod
+    def local_search(td: TensorDict, actions: torch.Tensor, max_iterations: int = 1000, **kwargs) -> torch.Tensor:
+        """cvrp/env.py:248-252 -> cvrp/local_search.py, with the project's own relocate / swap / 2-opt / 2-opt* search
+        (co_cvrp_local_search, corollout.h) in place of HGS-CVRP's SWAP*.  Reads td["locs"] (depot first), "demand",
+        "vehicle_capacity" and td["distances"] (float32 [B, N+1, N+1], used as given) when present.  The result has the
+        reference's layout: routes separated by one 0, no leading 0, trimmed to the batch's longest row; a row that
+        fails the reference's capacity check gets its original actions back (cvrp/local_search.py:82-96).  Other
+        keywords are ignored, as in the reference.  Returns an int64 tensor on td.device."""
+        del kwargs
+        locs = td["locs"]
+        if not locs.is_cuda:
+            raise NotImplementedError(f"FusedCVRPEnv.local_search runs on CUDA tensors only (got device {locs.device})")
+        if len(td.batch_size) > 1:
+            raise ValueError(f"local_search takes a batch with one dimension, got batch_size {tuple(td.batch_size)}")
+        distances = td.get("distances", None)
+        if distances is not None and distances.dtype != torch.float32:
+            raise ValueError(f"distances must be float32, got {distances.dtype}")
+        demand = td["demand"]
+        B = demand.shape[0]
+        if actions.dim() != 2 or actions.shape[0] != B:
+            raise ValueError(f"actions must be [{B}, T], got {tuple(actions.shape)}")
+        tours = actions.to(device=locs.device, dtype=torch.int64).contiguous()
+        its = torch.empty(B, dtype=torch.int32, device=locs.device)
+        feasible = torch.empty(B, dtype=torch.int32, device=locs.device)
+        src = dict(locs=locs.to(torch.float32).contiguous()) if distances is None else dict(distances=distances.contiguous())
+        out, used = native.cvrp_local_search(tours, demand.to(torch.float32).contiguous(),
+                                             td["vehicle_capacity"].reshape(B).to(torch.float32).contiguous(),
+                                             max_iterations, iterations=its, feasible=feasible, **src)
+        assert not bool((its < 0).any()), "Invalid tour"
+        max_pos = int(used.max())
+        new = out[:, :max_pos]
+        invalid = feasible == 0
+        if bool(invalid.any()):
+            new[invalid] = 0
+            orig = tours[invalid]
+            orig_max_pos = int((orig != 0).nonzero()[:, 1].max()) + 1
+            if orig_max_pos > max_pos:
+                new = torch.nn.functional.pad(new, (0, orig_max_pos - max_pos))
+            new[invalid, :orig_max_pos] = orig[:, :orig_max_pos]
+        return new.to(td.device if td.device is not None else locs.device)
+
+    @staticmethod
     def load_data(fpath, batch_size=[]):
         """cvrp/env.py:179-186: normalise demand by capacity."""
         from .data import load_npz_to_tensordict
@@ -563,6 +604,10 @@ class FusedSDVRPEnv(FusedCVRPEnv):
     co_pointer_logits with the dynamic term, co_select_action, co_tour_length)."""
 
     name = "sdvrp"
+
+    def local_search(self, td: TensorDict, actions: torch.Tensor, **kwargs) -> torch.Tensor:
+        """Not provided: the CVRP search assumes each customer is visited once, which split deliveries break."""
+        return FusedEnvBase.local_search(self, td, actions, **kwargs)
 
     def _reset(self, td: TensorDict, batch_size=None) -> TensorDict:
         """sdvrp/env.py:84-108"""

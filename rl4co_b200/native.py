@@ -42,7 +42,7 @@ EXPORTS = [
     "co_cache_width", "co_rollout_max_nodes", "co_rollout", "co_reward_stats", "co_split_tf32", "co_gemm_tf32x3", "co_encoder_mha",
     "co_ffn_fused", "co_ffn_tile_weights", "co_ffn_tiled_weight_floats", "co_generate_uniform", "co_generate_demand", "co_dihedral8",
     "co_sdvrp_step", "co_sdvrp_action_mask", "co_attn_fwd", "co_attn_bwd", "co_instance_norm", "co_op_step", "co_op_action_mask", "co_op_reward", "co_pctsp_step", "co_pctsp_action_mask",
-    "co_tsp_two_opt", "co_generate_locs", "co_symmetric_augment",
+    "co_tsp_two_opt", "co_generate_locs", "co_symmetric_augment", "co_cvrp_local_search",
 ]
 
 
@@ -157,6 +157,7 @@ def lib() -> ctypes.CDLL:
     L.co_sdvrp_step.argtypes = [c_void_p] * 9 + [c_int, c_int, c_void_p]
     L.co_check_tours.argtypes = [c_void_p] * 4 + [c_int] * 4 + [c_void_p]
     L.co_tsp_two_opt.argtypes = [c_void_p] * 5 + [c_int] * 3 + [c_void_p]
+    L.co_cvrp_local_search.argtypes = [c_void_p] * 9 + [c_int] * 4 + [c_void_p]
     L.co_reward_stats.argtypes = [c_void_p, c_void_p, c_int, c_void_p]
     L.co_op_action_mask.argtypes = [c_void_p] * 6 + [c_int, c_int, c_void_p]
     L.co_op_step.argtypes = [c_void_p] * 12 + [c_int, c_int, c_void_p]
@@ -402,6 +403,41 @@ def tsp_two_opt(tours, max_iterations: int = 1000, locs=None, distances=None, it
                                 _ptr(out, I64, "tours_out"), _ptr(iterations, I32, "iterations"), B, N,
                                 min(int(max_iterations), 2**31 - 1), _stream()), "co_tsp_two_opt")
     return out
+
+
+@_on_device_of_first_tensor
+def cvrp_local_search(tours, demand, capacity, max_iterations: int, locs=None, distances=None, iterations=None,
+                      feasible=None):
+    """co_cvrp_local_search: relocate / swap / 2-opt / 2-opt* local search of int64 tours [B, T] in the action format
+    (0 = depot) -> (tours [B, 2N] int64, used length [B] int32).  demand [B, N] and capacity [B] are float32; exactly
+    one of `locs` [B, N+1, 2] / `distances` [B, N+1, N+1] (float32) gives the distances.  `iterations` (moves applied,
+    -1 for a row that is not a visit of every customer) and `feasible` (1 when the result passes the reference's
+    capacity rule) are optional int32 [B] outputs."""
+    if (locs is None) == (distances is None):
+        raise ValueError("cvrp_local_search: pass exactly one of locs / distances")
+    if tours.dim() != 2:
+        raise ValueError(f"tours: expected [B, T], got {tuple(tours.shape)}")
+    B, T = tours.shape
+    if demand.dim() != 2 or demand.shape[0] != B:
+        raise ValueError(f"demand: expected [{B}, N], got {tuple(demand.shape)}")
+    N = demand.shape[1]
+    if tuple(capacity.shape) != (B,):
+        raise ValueError(f"capacity: expected [{B}], got {tuple(capacity.shape)}")
+    if locs is not None and tuple(locs.shape) != (B, N + 1, 2):
+        raise ValueError(f"locs: expected [{B}, {N + 1}, 2], got {tuple(locs.shape)}")
+    if distances is not None and tuple(distances.shape) != (B, N + 1, N + 1):
+        raise ValueError(f"distances: expected [{B}, {N + 1}, {N + 1}], got {tuple(distances.shape)}")
+    for name, t in (("iterations", iterations), ("feasible", feasible)):
+        if t is not None and tuple(t.shape) != (B,):
+            raise ValueError(f"{name}: expected [{B}], got {tuple(t.shape)}")
+    out = torch.empty(B, 2 * N, dtype=I64, device=tours.device)
+    used = torch.empty(B, dtype=I32, device=tours.device)
+    _check(lib().co_cvrp_local_search(_ptr(locs, F32, "locs"), _ptr(distances, F32, "distances"),
+                                      _ptr(demand, F32, "demand"), _ptr(capacity, F32, "capacity"),
+                                      _ptr(tours, I64, "tours"), _ptr(out, I64, "tours_out"), _ptr(used, I32, "used"),
+                                      _ptr(iterations, I32, "iterations"), _ptr(feasible, I32, "feasible"), B, N, T,
+                                      min(int(max_iterations), 2**31 - 1), _stream()), "co_cvrp_local_search")
+    return out, used
 
 
 @_on_device_of_first_tensor

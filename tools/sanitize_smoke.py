@@ -86,3 +86,20 @@ for B, S, N in ((37, 3, 1), (5, 8, 20), (3, 2, 1000)):
     native.symmetric_augment(torch.rand(B, N, 2, device=dev), torch.rand(S * B, device=dev) * 4 * torch.pi, S)
 torch.cuda.synchronize()
 print("symmetric_augment ok")
+# CVRP local search (co_cvrp_local_search): both distance sources on both sides of the residency bound, an invalid row
+# (copied through) and the pointer surgery of every move kind
+for n in (20, 223, 300):
+    g = torch.Generator().manual_seed(n)
+    locs = torch.rand(4, n + 1, 2, generator=g).to(dev)
+    dem = (torch.randint(1, 10, (4, n), generator=g) / 40.0).to(dev)
+    perm = torch.argsort(torch.rand(4, n, generator=g), dim=1) + 1
+    tours = torch.zeros(4, 2 * n, dtype=torch.int64)
+    tours[:, ::2] = perm  # one customer per route
+    tours[3, 0] = n + 1
+    tours = tours.to(dev)
+    d = (locs[:, :, None] - locs[:, None]).norm(dim=-1)
+    its = torch.empty(4, dtype=torch.int32, device=dev)
+    native.cvrp_local_search(tours, dem, torch.ones(4, device=dev), 50, locs=locs, iterations=its)
+    native.cvrp_local_search(tours, dem, torch.ones(4, device=dev), 50, distances=d, iterations=its)
+torch.cuda.synchronize()
+print("cvrp local search ok")
