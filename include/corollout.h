@@ -299,6 +299,50 @@ typedef struct co_rollout_args {
   const float* node_limit;
 } co_rollout_args;
 
+/* Efficient active search, embedding variant (EAS-Emb; rl4co/models/zoo/eas/search.py:198-235): gradient of a
+ * weighted sum of trajectory log-likelihoods with respect to the folded logit key Lf = L W_out (block 2 of the cache).
+ *   Row j = r * B_inst + b (r < num_rows, start-major as co_rollout) is a trajectory of instance b: actions [R*B_inst, T]
+ *   int64, column 0 a forced first action (tsp: any node, cvrp: a customer) with log-prob 0, as a multistart start;
+ *   columns after the episode is done are padding and are not read.  Each step t >= 1 is replayed as co_rollout in
+ *   evaluate mode: query = graph_ctx + current-node table row (tsp: + the first-node table row of column 0; cvrp:
+ *   + (capacity - used) * w_capacity), masked 8-head glimpse -> head output o_t [E], u_n = o_t . Lf[n] / sqrt(E),
+ *   z_n = C tanh(u_n) / temperature (masked: -inf), logp = log_softmax(z).  Outputs:
+ *     loglik[j] = sum_t logp_t[a_t]
+ *     dLf[b, n, :] = sum over the rows j of b and their steps t of  g_{j,t,n} o_{j,t},
+ *       g_{j,t,n} = coef[j] (delta_{n,a_t} - p_{t,n}) / temperature * C (1 - tanh^2(u_n)) / sqrt(E)  (0 if n is masked)
+ *     i.e. dLf = d(sum_j coef[j] loglik[j]) / dLf.
+ *   One CTA owns one instance; every dLf entry is summed in the fixed order (row, step) by one thread, so the result is
+ *   bit-identical across launches and does not depend on the other instances of the batch.  No placeholder query is
+ *   needed: column 0 is always forced.
+ *   A row whose column 0 is out of range, that takes an action the replayed mask forbids (or outside [0, N)), or that
+ *   is not done within min(T, 2 * 32 * ceil(N / 32)) columns contributes nothing, gets loglik = NaN and adds 1 to
+ *   *bad_rows (device int32, caller-zeroed, nullable).
+ *   cache: tsp the 5E layout (first-node table; the 4E layout is CO_ERR_UNSUPPORTED), cvrp 4E; 16-byte aligned.
+ *   Errors: env other than tsp / cvrp, N > co_rollout_max_nodes() or tanh_clipping <= 0: CO_ERR_UNSUPPORTED; null
+ *   pointers, B_inst < 0, N < 2, num_rows < 1, T < 1 (tsp: T < N), temperature <= 0, a wrong cvrp cache width,
+ *   missing cvrp demand / w_capacity or misaligned cache / dLf: CO_ERR_BAD_ARG. */
+typedef struct co_eas_grad_args {
+  int32_t env_kind;          /* CO_ENV_TSP | CO_ENV_CVRP                                  */
+  int32_t B_inst;            /* instances (cache rows)                                   */
+  int32_t num_rows;          /* R trajectories per instance                              */
+  int32_t N;                 /* nodes incl. depot                                        */
+  int32_t T;                 /* columns of actions                                       */
+  int32_t cache_width;       /* floats per cache row: tsp 5E, cvrp 4E                    */
+  float tanh_clipping;       /* C                                                        */
+  float temperature;
+  const float* cache;        /* [B_inst, N, cache_width]                                 */
+  const float* graph_ctx;    /* [B_inst, E] or NULL                                      */
+  const float* w_capacity;   /* [E] cvrp                                                 */
+  const float* demand;       /* [B_inst, N-1] cvrp                                       */
+  const float* vehicle_capacity; /* [B_inst] cvrp or NULL (= 1.0)                        */
+  const int64_t* actions;    /* [R * B_inst, T]                                          */
+  const float* coef;         /* [R * B_inst]                                             */
+  float* dLf;                /* [B_inst, N, E] out                                       */
+  float* loglik;             /* [R * B_inst] out                                         */
+  int32_t* bad_rows;         /* [1] out (accumulated) or NULL                            */
+} co_eas_grad_args;
+int co_eas_key_grad(const co_eas_grad_args* args, void* stream);
+
 int co_cache_width(int env_kind); /* floats per node row of the widest rollout cache layout (tsp 5E, cvrp 4E) */
 /* largest N the persistent kernel is instantiated for (else CO_ERR_UNSUPPORTED) */
 int co_rollout_max_nodes(void);

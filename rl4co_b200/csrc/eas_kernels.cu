@@ -1,0 +1,444 @@
+// co_eas_key_grad: gradient of a weighted sum of trajectory log-likelihoods with respect to the folded pointer logit
+// key (block 2 of the rollout cache), for efficient active search with embedding updates (EAS-Emb, Hottung et al.
+// 2022; rl4co/models/zoo/eas).  See include/corollout.h for the formula and the argument rules.
+//
+// Design: one CTA (256 threads = 8 warps) owns one instance and replays its R trajectories one after the other,
+// teacher-forced, with the step semantics of the rollout kernel in evaluate mode (rollout_impl.cuh).
+//   * warp h = head h.  Lane l owns nodes n = 32 k + l (k < SPL): their head-h glimpse key / value slices live in
+//     registers; the folded key Lf (head-major) and the fp32 gradient accumulator (private to the owning thread)
+//     live in shared memory, so no entry of dLf is ever written by two threads and no atomics are used.
+//   * per step every warp forms its 16 query channels (fixed part + the current-node table row, read from L2 one step
+//     ahead because the actions are known; cvrp: + remaining capacity x w_capacity), runs its masked glimpse head,
+//     writes the normalised head output o_t[16h..16h+15] and its share of every pointer logit; one block barrier;
+//     warp 0 then sums the eight shares in a fixed order, applies tanh clip / mask / temperature, the log-softmax
+//     and writes g_{t,n} = coef (delta_{n,a} - p_n) / T * C (1 - tanh^2) / sqrt(E) for the step.
+//   * o_t and g_t are buffered for Q steps (two halves, so the other warps run ahead into the next glimpse while warp
+//     0 finishes a step); a full half is folded into the accumulator as one rank-Q update, q ascending: the summation
+//     order is fixed by (row, step) alone, so the result does not depend on the launch or the batch it is part of.
+//   * the environment state (visited set, cvrp load and depot rule) is replicated in every thread as 128-bit masks, so
+//     every thread can validate a whole row before it is replayed: a row holding an infeasible action contributes
+//     nothing, gets loglik = NaN and is counted in *bad_rows.
+#include "rollout_impl.cuh"
+
+namespace co {
+namespace {
+
+constexpr int EAS_Q = 8;  // steps per rank-Q update (half of the o / g ring)
+
+template <int SPL>
+struct EasSmem {
+  static constexpr int NS = 32 * SPL;
+  float4 lf[8 * 4 * NS];               // folded key, [head][chunk of 4 channels][node]
+  float4 acc[8 * SPL * 4 * 32];        // gradient accumulator, [head][k][chunk][lane]: thread-private entries
+  float tile[8][32 * TILE_LD];         // per-warp transpose tile for the value reduction
+  alignas(16) float obuf[2 * EAS_Q][E];    // head outputs o_t of the buffered steps
+  alignas(16) float gbuf[2 * EAS_Q][NS];   // residuals g_t of the buffered steps (0 for masked / padding nodes)
+  alignas(16) float part[2][8][NS];        // per-head share of every pointer logit, double-buffered by step parity
+  alignas(16) float qh[8][D];              // per-warp query slice
+  float qfix[E];                           // per-row fixed part of the query
+  float wcap[E];                           // cvrp: remaining-capacity column of project_context
+  float dem[NS];                           // cvrp: demand per node (depot 0)
+  unsigned char order[NS];                 // cvrp: customers sorted by demand (ascending)
+  unsigned char rank_of[NS];               // cvrp: demand rank of each customer
+  short acts[2 * NS];                      // the row's actions (the first 2 NS columns)
+};
+
+// Environment state of one trajectory, replicated in every thread (tsp/env.py:60-86, cvrp/env.py:66-136 as
+// rollout_impl.cuh replays them).
+// word w of a 128-bit mask held as four scalars (selects, not an indexed array, so the masks stay in registers)
+__device__ __forceinline__ uint32_t word4(const uint4& m, int w) {
+  return w == 0 ? m.x : (w == 1 ? m.y : (w == 2 ? m.z : m.w));
+}
+__device__ __forceinline__ void set4(uint4& m, int i) {
+  const uint32_t bit = 1u << (i & 31), w = (uint32_t)i >> 5;
+  m.x |= w == 0 ? bit : 0u; m.y |= w == 1 ? bit : 0u; m.z |= w == 2 ? bit : 0u; m.w |= w == 3 ? bit : 0u;
+}
+__device__ __forceinline__ uint32_t rank_preset(int nc, int lo) {  // bits >= #customers preset
+  return (nc >= lo + 32) ? 0u : (nc <= lo ? 0xffffffffu : (0xffffffffu << (nc - lo)));
+}
+
+template <int ENV>
+struct EasEnv {
+  uint4 vis;    // visited nodes
+  uint4 rmask;  // cvrp: visited customers by demand rank
+  int cur, t, nvis;
+  float used;
+  bool depot_seen, anyfeas, done;
+
+  __device__ __forceinline__ void reset(int N) {
+    vis = make_uint4(0u, 0u, 0u, 0u);
+    rmask = make_uint4(rank_preset(N - 1, 0), rank_preset(N - 1, 32), rank_preset(N - 1, 64), rank_preset(N - 1, 96));
+    cur = 0; t = 0; nvis = 0; used = 0.f;
+    depot_seen = false; anyfeas = false; done = false;
+  }
+  __device__ __forceinline__ bool visited(int n) const { return (word4(vis, n >> 5) >> (n & 31)) & 1u; }
+  __device__ __forceinline__ bool feasible(int n, const float* dem, float thr) const {
+    if (ENV == CO_ENV_TSP) return !visited(n);
+    if (n == 0) return !(cur == 0 && anyfeas);
+    return !visited(n) && !((dem[n] + used) > thr);
+  }
+  __device__ __forceinline__ void step(int a, int N, const float* dem, const unsigned char* order,
+                                       const unsigned char* rank_of, float thr) {
+    if (ENV == CO_ENV_TSP) {
+      set4(vis, a);
+      cur = a; ++t;
+      done = t >= N;
+      return;
+    }
+    used = (used + dem[a == 0 ? 1 : a]) * (a != 0 ? 1.0f : 0.0f);
+    nvis += (a != 0 || !depot_seen) ? 1 : 0;
+    depot_seen = depot_seen || (a == 0);
+    if (a != 0) {
+      set4(vis, a);
+      set4(rmask, rank_of[a]);
+    }
+    // depot rule (cvrp/env.py:134): an unvisited customer fits <=> the unvisited customer of least demand fits
+    int pmin = 128;
+    if (~rmask.w) pmin = 96 + __ffs(~rmask.w) - 1;
+    if (~rmask.z) pmin = 64 + __ffs(~rmask.z) - 1;
+    if (~rmask.y) pmin = 32 + __ffs(~rmask.y) - 1;
+    if (~rmask.x) pmin = __ffs(~rmask.x) - 1;
+    anyfeas = (pmin < N - 1) && !((dem[order[pmin < N - 1 ? pmin : 0]] + used) > thr);
+    cur = a; ++t;
+    done = nvis >= N;
+  }
+};
+
+template <int SPL, int ENV>
+__global__ void __launch_bounds__(256, 1) eas_key_grad_kernel(const co_eas_grad_args A) {
+  constexpr int NS = 32 * SPL;
+  constexpr int CW = (ENV == CO_ENV_TSP ? 5 : 4) * E;  // tsp: the 5E layout with the first-node table
+  constexpr int CUR_BLK = CW / E - 1;
+  constexpr bool VRP = ENV == CO_ENV_CVRP;
+  constexpr float LOG2E = 1.4426950408889634f, INV_SQRT_E = 0.08838834764831845f;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  EasSmem<SPL>& sm = *reinterpret_cast<EasSmem<SPL>*>(smem_raw);
+
+  const int tid = threadIdx.x, lane = tid & 31, h = tid >> 5;
+  const int N = A.N, B_inst = A.B_inst, R = A.num_rows, T = A.T;
+  const int TB = T < 2 * NS ? T : 2 * NS;  // columns read: a feasible episode ends within 2 (N - 1) steps
+  const float clip = A.tanh_clipping, inv_temp = 1.0f / A.temperature;
+  const float gscale = clip * inv_temp * INV_SQRT_E;
+  float* tile = sm.tile[h];
+
+  float2 Kr[SPL][8], Vr[SPL][8];
+  int ps = 0;  // global step parity (part[] buffer)
+
+  for (int b = blockIdx.x; b < B_inst; b += gridDim.x) {
+    __syncthreads();  // the previous instance is done with shared memory
+    const float* crow = A.cache + (size_t)b * N * CW;
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) {
+      const int n = 32 * k + lane;
+      if (n < N) {
+        const float4* ks = reinterpret_cast<const float4*>(crow + (size_t)n * CW + 0 * E + h * D);
+        const float4* vs = reinterpret_cast<const float4*>(crow + (size_t)n * CW + 1 * E + h * D);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const float4 kv = __ldg(ks + c), vv = __ldg(vs + c);
+          Kr[k][2 * c] = make_float2(kv.x, kv.y); Kr[k][2 * c + 1] = make_float2(kv.z, kv.w);
+          Vr[k][2 * c] = make_float2(vv.x, vv.y); Vr[k][2 * c + 1] = make_float2(vv.z, vv.w);
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { Kr[k][j] = make_float2(0.f, 0.f); Vr[k][j] = make_float2(0.f, 0.f); }
+      }
+    }
+    for (int i = tid; i < 8 * 4 * NS; i += 256) {  // folded key, head-major; zero rows for padding nodes
+      const int n = i % NS, hc = i / NS;
+      sm.lf[i] = n < N ? __ldg(reinterpret_cast<const float4*>(crow + (size_t)n * CW + 2 * E) + hc)
+                       : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    for (int i = tid; i < 8 * SPL * 4 * 32; i += 256) sm.acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (tid < E) sm.wcap[tid] = VRP ? A.w_capacity[tid] : 0.f;
+    if (tid < NS) sm.dem[tid] = (VRP && tid >= 1 && tid < N) ? A.demand[(size_t)b * (N - 1) + tid - 1] : 0.f;
+    const float cap = (VRP && A.vehicle_capacity) ? A.vehicle_capacity[b] : 1.0f;
+    const float thr = cap + 1e-5f;  // fp32 add, as `td["vehicle_capacity"] + 1e-5`
+    __syncthreads();
+    if (VRP) {  // rank-sort customers by demand (ties by index), as rollout_impl.cuh
+      if (tid >= 1 && tid < N) {
+        const float d = sm.dem[tid];
+        int rank = 0;
+        for (int m = 1; m < N; ++m) {
+          const float dm = sm.dem[m];
+          rank += (dm < d || (dm == d && m < tid)) ? 1 : 0;
+        }
+        sm.order[rank] = (unsigned char)tid;
+        sm.rank_of[tid] = (unsigned char)rank;
+      }
+    }
+
+    int hb = 0, cnt = 0;  // ring half being filled, steps buffered in it
+    // rank-cnt update of this thread's accumulator entries from ring half `half`
+    auto flush = [&](int half, int nq) {
+#pragma unroll
+      for (int k = 0; k < SPL; ++k) {
+        float4* ap = sm.acc + ((h * SPL + k) * 4) * 32 + lane;
+        float4 a0 = ap[0], a1 = ap[32], a2 = ap[64], a3 = ap[96];
+        for (int q = 0; q < nq; ++q) {
+          const int sl = half * EAS_Q + q;
+          const float g = sm.gbuf[sl][32 * k + lane];
+          const float4* o = reinterpret_cast<const float4*>(sm.obuf[sl] + h * D);
+          const float4 o0 = o[0], o1 = o[1], o2 = o[2], o3 = o[3];
+          a0.x = fmaf(g, o0.x, a0.x); a0.y = fmaf(g, o0.y, a0.y); a0.z = fmaf(g, o0.z, a0.z); a0.w = fmaf(g, o0.w, a0.w);
+          a1.x = fmaf(g, o1.x, a1.x); a1.y = fmaf(g, o1.y, a1.y); a1.z = fmaf(g, o1.z, a1.z); a1.w = fmaf(g, o1.w, a1.w);
+          a2.x = fmaf(g, o2.x, a2.x); a2.y = fmaf(g, o2.y, a2.y); a2.z = fmaf(g, o2.z, a2.z); a2.w = fmaf(g, o2.w, a2.w);
+          a3.x = fmaf(g, o3.x, a3.x); a3.y = fmaf(g, o3.y, a3.y); a3.z = fmaf(g, o3.z, a3.z); a3.w = fmaf(g, o3.w, a3.w);
+        }
+        ap[0] = a0; ap[32] = a1; ap[64] = a2; ap[96] = a3;
+      }
+    };
+
+    for (int r = 0; r < R; ++r) {
+      const size_t row = (size_t)r * B_inst + b;  // start-major, as co_rollout
+      __syncthreads();  // every thread is done with the previous row's actions
+      for (int c = tid; c < TB; c += 256) {
+        const int64_t a = A.actions[row * T + c];
+        sm.acts[c] = (short)((a < 0 || a >= N) ? -1 : a);
+      }
+      __syncthreads();
+      const float coef = A.coef[row];
+
+      // ---- validation: every thread replays the row's mask (uniform result, no communication)
+      EasEnv<ENV> env;
+      env.reset(N);
+      bool bad = sm.acts[0] < (VRP ? 1 : 0);  // column 0: the forced start (cvrp: a customer)
+      if (!bad) {
+        env.step(sm.acts[0], N, sm.dem, sm.order, sm.rank_of, thr);
+        while (!env.done) {
+          if (env.t >= TB) { bad = true; break; }
+          const int a = sm.acts[env.t];
+          if (a < 0 || !env.feasible(a, sm.dem, thr)) { bad = true; break; }
+          env.step(a, N, sm.dem, sm.order, sm.rank_of, thr);
+        }
+      }
+      if (bad) {
+        if (tid == 0) {
+          A.loglik[row] = __int_as_float(0x7fc00000);
+          if (A.bad_rows) atomicAdd(A.bad_rows, 1);
+        }
+        continue;
+      }
+
+      // ---- replay
+      env.reset(N);
+      const int a0 = sm.acts[0];
+      env.step(a0, N, sm.dem, sm.order, sm.rank_of, thr);
+      if (tid < E) {  // fixed part of the query: graph context (+ tsp: the first-node table row, context.py:129-133)
+        float g = A.graph_ctx ? A.graph_ctx[(size_t)b * E + tid] : 0.f;
+        if (ENV == CO_ENV_TSP) g += __ldg(crow + (size_t)a0 * CW + 3 * E + tid);
+        sm.qfix[tid] = g;
+      }
+      __syncthreads();
+      float ll = 0.f;  // lane 0 of warp 0
+      float pt = lane < D ? __ldg(crow + (size_t)env.cur * CW + CUR_BLK * E + h * D + lane) : 0.f;
+      while (!env.done) {
+        const int a = sm.acts[env.t];
+        const int sl = hb * EAS_Q + cnt;
+        float* part = sm.part[ps][h];
+        // next step's current-node table row (the action of this step), in flight during this step
+        const float pt_next = lane < D ? __ldg(crow + (size_t)a * CW + CUR_BLK * E + h * D + lane) : 0.f;
+        // ---------------- glimpse head h, head output, share of head h in every pointer logit
+        {
+          if (lane < D) {
+            float q = sm.qfix[h * D + lane] + pt;
+            if (VRP) q = fmaf(cap - env.used, sm.wcap[h * D + lane], q);  // context.py:147-149
+            sm.qh[h][lane] = q;
+          }
+          __syncwarp();
+          const float4* qp = reinterpret_cast<const float4*>(sm.qh[h]);
+          float2 sc2[SPL];
+#pragma unroll
+          for (int k = 0; k < SPL; ++k) sc2[k] = make_float2(0.f, 0.f);
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const float4 x = qp[c];
+#pragma unroll
+            for (int k = 0; k < SPL; ++k) {
+              sc2[k] = ffma2(make_float2(x.x, x.y), Kr[k][2 * c], sc2[k]);
+              sc2[k] = ffma2(make_float2(x.z, x.w), Kr[k][2 * c + 1], sc2[k]);
+            }
+          }
+          float sc[SPL], m = -INFINITY;
+          bool fz[SPL];
+#pragma unroll
+          for (int k = 0; k < SPL; ++k) {
+            const int n = 32 * k + lane;
+            fz[k] = n < N && env.feasible(n, sm.dem, thr);
+            sc[k] = fz[k] ? (sc2[k].x + sc2[k].y) * (0.25f * LOG2E) : -INFINITY;
+            m = fmaxf(m, sc[k]);
+          }
+          m = funkey(__reduce_max_sync(FULL, fkey(m)));
+          float2 acc[8];
+          float esum = 0.f;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) acc[j] = make_float2(0.f, 0.f);
+#pragma unroll
+          for (int k = 0; k < SPL; ++k) {
+            const float e = fz[k] ? ex2(sc[k] - m) : 0.f;
+            esum += e;
+            const float2 e2 = make_float2(e, e);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) acc[j] = ffma2(e2, Vr[k][j], acc[j]);
+          }
+          float4* trow = reinterpret_cast<float4*>(tile + lane * TILE_LD);
+#pragma unroll
+          for (int c = 0; c < 4; ++c) trow[c] = make_float4(acc[2 * c].x, acc[2 * c].y, acc[2 * c + 1].x, acc[2 * c + 1].y);
+          esum = warp_sum_fixed(esum);
+          __syncwarp();
+          const int d = lane & 15, half = lane >> 4;
+          float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+#pragma unroll
+          for (int rr = 0; rr < 16; rr += 4) {
+            s0 += tile[(16 * half + ((rr + 0 + 4 * half) & 15)) * TILE_LD + d];
+            s1 += tile[(16 * half + ((rr + 1 + 4 * half) & 15)) * TILE_LD + d];
+            s2 += tile[(16 * half + ((rr + 2 + 4 * half) & 15)) * TILE_LD + d];
+            s3 += tile[(16 * half + ((rr + 3 + 4 * half) & 15)) * TILE_LD + d];
+          }
+          float o = (s0 + s1) + (s2 + s3);
+          o += __shfl_xor_sync(FULL, o, 16);
+          if (lane < 16) sm.obuf[sl][h * D + lane] = o / esum;
+          __syncwarp();
+          const float4* op = reinterpret_cast<const float4*>(sm.obuf[sl] + h * D);
+          const float4 o0 = op[0], o1 = op[1], o2 = op[2], o3 = op[3];
+#pragma unroll
+          for (int k = 0; k < SPL; ++k) {
+            const float4* lp = sm.lf + (h * 4) * NS + 32 * k + lane;
+            const float4 l0 = lp[0], l1 = lp[NS], l2 = lp[2 * NS], l3 = lp[3 * NS];
+            float2 p2 = make_float2(0.f, 0.f);
+            p2 = ffma2(make_float2(o0.x, o0.y), make_float2(l0.x, l0.y), p2);
+            p2 = ffma2(make_float2(o0.z, o0.w), make_float2(l0.z, l0.w), p2);
+            p2 = ffma2(make_float2(o1.x, o1.y), make_float2(l1.x, l1.y), p2);
+            p2 = ffma2(make_float2(o1.z, o1.w), make_float2(l1.z, l1.w), p2);
+            p2 = ffma2(make_float2(o2.x, o2.y), make_float2(l2.x, l2.y), p2);
+            p2 = ffma2(make_float2(o2.z, o2.w), make_float2(l2.z, l2.w), p2);
+            p2 = ffma2(make_float2(o3.x, o3.y), make_float2(l3.x, l3.y), p2);
+            p2 = ffma2(make_float2(o3.z, o3.w), make_float2(l3.z, l3.w), p2);
+            part[32 * k + lane] = p2.x + p2.y;
+          }
+        }
+        __syncthreads();  // every head's share of every logit is in shared memory
+
+        if (h == 0) {
+          // ---------------- pointer logits, heads summed in fixed order; tanh clip, mask, temperature, log-softmax
+          const float(*pp)[NS] = sm.part[ps];
+          float z[SPL], th[SPL], m = -INFINITY;
+          bool fz[SPL];
+#pragma unroll
+          for (int k = 0; k < SPL; ++k) {
+            const int n = 32 * k + lane;
+            const float u = ((pp[0][n] + pp[1][n]) + (pp[2][n] + pp[3][n])) + ((pp[4][n] + pp[5][n]) + (pp[6][n] + pp[7][n]));
+            fz[k] = n < N && env.feasible(n, sm.dem, thr);
+            th[k] = tanhf(u * INV_SQRT_E);
+            z[k] = fz[k] ? th[k] * clip * inv_temp : -INFINITY;
+            m = fmaxf(m, z[k]);
+          }
+          m = funkey(__reduce_max_sync(FULL, fkey(m)));
+          float e[SPL], s = 0.f;
+#pragma unroll
+          for (int k = 0; k < SPL; ++k) {
+            e[k] = fz[k] ? __expf(z[k] - m) : 0.f;
+            s += e[k];
+          }
+          s = warp_sum_fixed(s);  // 1 <= s <= N; order independent
+          const float inv_s = 1.0f / s;
+          float za = 0.f;
+#pragma unroll
+          for (int k = 0; k < SPL; ++k) {
+            const int n = 32 * k + lane;
+            za = (n == a) ? z[k] : za;
+            const float g = fz[k] ? coef * (((n == a) ? 1.0f : 0.0f) - e[k] * inv_s) * gscale * (1.0f - th[k] * th[k]) : 0.f;
+            sm.gbuf[sl][n] = g;
+          }
+          za = __shfl_sync(FULL, za, a & 31);
+          if (lane == 0) {
+            const float lp = (za - m) - logf(s);
+            ll += lp;
+          }
+        }
+        // ---------------- environment step (replicated)
+        env.step(a, N, sm.dem, sm.order, sm.rank_of, thr);
+        pt = pt_next;
+        ps ^= 1;
+        if (++cnt == EAS_Q || env.done) {
+          __syncthreads();  // warp 0's residuals of the last step are in shared memory
+          flush(hb, cnt);
+          hb ^= 1;
+          cnt = 0;
+        }
+      }
+      if (tid == 0) A.loglik[row] = ll;
+    }
+
+    // ---- dLf rows of this instance (thread-private accumulator entries)
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) {
+      const int n = 32 * k + lane;
+      if (n < N) {
+        const float4* ap = sm.acc + ((h * SPL + k) * 4) * 32 + lane;
+        float4* dst = reinterpret_cast<float4*>(A.dLf + ((size_t)b * N + n) * E + h * D);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) dst[c] = ap[32 * c];
+      }
+    }
+  }
+}
+
+template <int SPL, int ENV>
+int launch_eas(const co_eas_grad_args& A, cudaStream_t st) {
+  auto kern = eas_key_grad_kernel<SPL, ENV>;
+  const size_t smem = sizeof(EasSmem<SPL>);
+  static PerDeviceOnce once;
+  static int ctas_per_sm = 1;
+  bool& configured = once.flag();
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return fail(CO_ERR_CUDA, "co_eas_key_grad: smem attribute: %s", cudaGetErrorString(e));
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern, 256, smem);
+    if (e != cudaSuccess || ctas_per_sm < 1) return fail(CO_ERR_CUDA, "co_eas_key_grad: occupancy query failed%s");
+    configured = true;
+  }
+  int grid = device_info().sm_count * ctas_per_sm;
+  if (grid > A.B_inst) grid = A.B_inst;
+  kern<<<grid, 256, smem, st>>>(A);
+  return check_launch("co_eas_key_grad");
+}
+
+template <int ENV>
+int dispatch_eas(const co_eas_grad_args& A, cudaStream_t st) {
+  if (A.N <= 32) return launch_eas<1, ENV>(A, st);
+  if (A.N <= 64) return launch_eas<2, ENV>(A, st);
+  return launch_eas<4, ENV>(A, st);
+}
+
+}  // namespace
+}  // namespace co
+
+using namespace co;
+
+extern "C" int co_eas_key_grad(const co_eas_grad_args* args, void* stream) {
+  if (!args) return fail(CO_ERR_BAD_ARG, "co_eas_key_grad: null args%s");
+  const co_eas_grad_args& A = *args;
+  if (A.env_kind != CO_ENV_TSP && A.env_kind != CO_ENV_CVRP)
+    return fail(CO_ERR_UNSUPPORTED, "co_eas_key_grad: env kind %s%lld (tsp and cvrp only)", "", A.env_kind);
+  if (!A.cache || !A.actions || !A.coef || !A.dLf || !A.loglik)
+    return fail(CO_ERR_BAD_ARG, "co_eas_key_grad: null pointer%s");
+  if (A.B_inst < 0 || A.N < 2 || A.num_rows < 1 || A.T < 1)
+    return fail(CO_ERR_BAD_ARG, "co_eas_key_grad: bad shape%s B=%lld N=%lld", "", A.B_inst, A.N);
+  if (A.N > co_rollout_max_nodes()) return fail(CO_ERR_UNSUPPORTED, "co_eas_key_grad: N=%s%lld > 128 nodes", "", A.N);
+  if (!(A.temperature > 0.f)) return fail(CO_ERR_BAD_ARG, "co_eas_key_grad: temperature must be > 0%s");
+  if (!(A.tanh_clipping > 0.f)) return fail(CO_ERR_UNSUPPORTED, "co_eas_key_grad: tanh_clipping must be > 0%s");
+  if (A.env_kind == CO_ENV_TSP) {
+    if (A.cache_width != 5 * E)
+      return fail(CO_ERR_UNSUPPORTED, "co_eas_key_grad: tsp needs the 5E cache (first-node table)%s");
+    if (A.T < A.N) return fail(CO_ERR_BAD_ARG, "co_eas_key_grad: T < N%s");
+  } else {
+    if (A.cache_width != 4 * E) return fail(CO_ERR_BAD_ARG, "co_eas_key_grad: cvrp cache_width must be 4E%s");
+    if (!A.demand || !A.w_capacity) return fail(CO_ERR_BAD_ARG, "co_eas_key_grad: demand / w_capacity required for cvrp%s");
+  }
+  const uintptr_t al = (uintptr_t)A.cache | (uintptr_t)A.dLf;
+  if (al & 15) return fail(CO_ERR_BAD_ARG, "co_eas_key_grad: cache / dLf must be 16-byte aligned%s");
+  if (A.B_inst == 0) return CO_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  return A.env_kind == CO_ENV_TSP ? dispatch_eas<CO_ENV_TSP>(A, st) : dispatch_eas<CO_ENV_CVRP>(A, st);
+}

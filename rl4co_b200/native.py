@@ -22,7 +22,7 @@ INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 LIB_PATH = os.path.join(_HERE, "libcorollout.so")
 SOURCES = ["abi.cu", "env_kernels.cu", "decode_step.cu", "rollout.cu", "rollout_tsp.cu", "rollout_cvrp.cu", "rollout_ms_tsp.cu", "rollout_ms_cvrp.cu", "rollout_sdvrp.cu", "rollout_op.cu", "rollout_pctsp.cu", "gemm_tf32x3.cu",
            "encoder_mha.cu", "encoder_mha_wgmma.cu",
-           "ffn_fused.cu", "data_kernels.cu", "attn_train.cu", "norm_kernels.cu", "op_kernels.cu", "local_search.cu"]
+           "ffn_fused.cu", "data_kernels.cu", "attn_train.cu", "norm_kernels.cu", "op_kernels.cu", "local_search.cu", "eas_kernels.cu"]
 HEADERS = ["co_common.cuh", "rollout_impl.cuh", "rollout_ms_impl.cuh", "wgmma.cuh"]
 
 CO_OK = 0
@@ -43,6 +43,7 @@ EXPORTS = [
     "co_ffn_fused", "co_ffn_tile_weights", "co_ffn_tiled_weight_floats", "co_generate_uniform", "co_generate_demand", "co_dihedral8",
     "co_sdvrp_step", "co_sdvrp_action_mask", "co_attn_fwd", "co_attn_bwd", "co_instance_norm", "co_op_step", "co_op_action_mask", "co_op_reward", "co_pctsp_step", "co_pctsp_action_mask",
     "co_tsp_two_opt", "co_generate_locs", "co_symmetric_augment", "co_cvrp_local_search",
+    "co_eas_key_grad",
 ]
 
 
@@ -68,6 +69,13 @@ class RolloutArgs(Structure):
         ("node_emb", c_void_p), ("w_first", c_void_p), ("cache_width", c_int32), ("reserved0", c_int32),
         ("dyn_w", c_void_p), ("node_limit", c_void_p),
     ]
+
+
+class EasGradArgs(Structure):
+    _fields_ = [("env_kind", c_int32), ("B_inst", c_int32), ("num_rows", c_int32), ("N", c_int32), ("T", c_int32),
+                ("cache_width", c_int32), ("tanh_clipping", c_float), ("temperature", c_float)] + [
+        (n, c_void_p) for n in ("cache", "graph_ctx", "w_capacity", "demand", "vehicle_capacity", "actions", "coef",
+                                "dLf", "loglik", "bad_rows")]
 
 
 class AttnArgs(Structure):
@@ -165,6 +173,7 @@ def lib() -> ctypes.CDLL:
     L.co_pctsp_step.argtypes = [c_void_p] * 11 + [c_int, c_int, c_void_p]
     L.co_op_reward.argtypes = [c_void_p] * 3 + [c_int, c_int, c_int, c_void_p]
     L.co_instance_norm.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_long, c_int, c_float, c_void_p]
+    L.co_eas_key_grad.argtypes = [POINTER(EasGradArgs), c_void_p]
     L.co_attn_fwd.argtypes = [POINTER(AttnArgs), c_void_p]
     L.co_attn_bwd.argtypes = [POINTER(AttnArgs), c_void_p]
     L.co_cache_width.argtypes = [c_int]
@@ -438,6 +447,52 @@ def cvrp_local_search(tours, demand, capacity, max_iterations: int, locs=None, d
                                       _ptr(iterations, I32, "iterations"), _ptr(feasible, I32, "feasible"), B, N, T,
                                       min(int(max_iterations), 2**31 - 1), _stream()), "co_cvrp_local_search")
     return out, used
+
+
+@_on_device_of_first_tensor
+def eas_key_grad(env_name, cache, actions, coef, graph_ctx=None, w_capacity=None, demand=None, vehicle_capacity=None,
+                 tanh_clipping=10.0, temperature=1.0, bad_rows=None):
+    """co_eas_key_grad: teacher-forced replay of R trajectories per instance -> (dLf [B_inst, N, E], loglik [R*B_inst])
+    with dLf = d(sum_j coef[j] loglik[j]) / d(folded logit key, block 2 of `cache`).  `cache` [B_inst, N, W] (tsp: 5E
+    layout, cvrp: 4E); actions [R*B_inst, T] int64 start-major with column 0 a forced start; coef [R*B_inst] float32.
+    An infeasible row gets loglik NaN and adds 1 to `bad_rows` (optional int32 [1] device counter); no host sync."""
+    if env_name not in ("tsp", "cvrp"):
+        raise NotImplementedError(f"co_eas_key_grad covers tsp and cvrp, not {env_name!r}")
+    if cache.dim() != 3:
+        raise ValueError(f"cache: expected [B_inst, N, W], got {tuple(cache.shape)}")
+    B_inst, N, W = cache.shape
+    if actions.dim() != 2 or B_inst == 0 or actions.shape[0] % max(B_inst, 1) or actions.shape[0] == 0:
+        raise ValueError(f"actions: expected [R * {B_inst}, T], got {tuple(actions.shape)}")
+    R, T = actions.shape[0] // B_inst, actions.shape[1]
+    if tuple(coef.shape) != (R * B_inst,):
+        raise ValueError(f"coef: expected [{R * B_inst}], got {tuple(coef.shape)}")
+    if graph_ctx is not None and tuple(graph_ctx.shape) != (B_inst, EMBED_DIM):
+        raise ValueError(f"graph_ctx: expected [{B_inst}, {EMBED_DIM}], got {tuple(graph_ctx.shape)}")
+    if env_name == "cvrp":
+        if w_capacity is None or demand is None:
+            raise ValueError("cvrp needs w_capacity and demand")
+        if tuple(w_capacity.shape) != (EMBED_DIM,) or tuple(demand.shape) != (B_inst, N - 1):
+            raise ValueError(f"w_capacity must be [{EMBED_DIM}] and demand [{B_inst}, {N - 1}]")
+        if vehicle_capacity is not None and tuple(vehicle_capacity.shape) != (B_inst,):
+            raise ValueError(f"vehicle_capacity: expected [{B_inst}], got {tuple(vehicle_capacity.shape)}")
+    if bad_rows is not None and tuple(bad_rows.shape) != (1,):
+        raise ValueError("bad_rows: expected an int32 [1] counter")
+    dLf = torch.empty(B_inst, N, EMBED_DIM, dtype=F32, device=cache.device)
+    loglik = torch.empty(R * B_inst, dtype=F32, device=cache.device)
+    a = EasGradArgs()
+    a.env_kind, a.B_inst, a.num_rows, a.N, a.T, a.cache_width = ENV_KIND[env_name], B_inst, R, N, T, W
+    a.tanh_clipping, a.temperature = float(tanh_clipping), float(temperature)
+    a.cache = _ptr(cache, F32, "cache")
+    a.graph_ctx = _ptr(graph_ctx, F32, "graph_ctx")
+    a.w_capacity = _ptr(w_capacity, F32, "w_capacity") if env_name == "cvrp" else None
+    a.demand = _ptr(demand, F32, "demand") if env_name == "cvrp" else None
+    a.vehicle_capacity = _ptr(vehicle_capacity, F32, "vehicle_capacity") if env_name == "cvrp" else None
+    a.actions = _ptr(actions, I64, "actions")
+    a.coef = _ptr(coef, F32, "coef")
+    a.dLf, a.loglik = _ptr(dLf, F32, "dLf"), _ptr(loglik, F32, "loglik")
+    a.bad_rows = _ptr(bad_rows, I32, "bad_rows")
+    _check(lib().co_eas_key_grad(ctypes.byref(a), _stream()), "co_eas_key_grad")
+    return dLf, loglik
 
 
 @_on_device_of_first_tensor
