@@ -22,8 +22,13 @@
 //     arg-max is REDUX.MAX + ballot (lowest node wins ties, torch semantics); sampling = arg-max of z - log q
 //     (Gumbel form of torch.multinomial's p/q); barrier 2; every thread merges the <= 4 per-warp winners.
 //   * the log-probability of the chosen node is NOT on the critical path: z of the last two steps stays in shared
-//     memory and a warp that has no logits work computes log-softmax(z)[a] of the PREVIOUS step while the others are
-//     in the tanh / arg-max phase (exact exp-sum with the tanh-clip bound as fixed offset, z <= clip/T).
+//     memory and two warps that have no logits work compute log-softmax(z)[a] while the others are in the tanh /
+//     arg-max phase (exact exp-sum with the tanh-clip bound as fixed offset, z <= clip/T), in two halves so that
+//     neither outlasts the selection: one takes the lane partials of the PREVIOUS step, the other the sum, log and
+//     store of the step before that.
+//   * what only the reward and the outputs need (action store, tour length, prize, penalties) is likewise done by
+//     another warp that is idle between the barriers, one step behind; the warps that gate barrier 1 replay only the
+//     state the next step's mask and context need.
 //   * the per-node context table (node_emb @ Wctx_cur^T) sits in shared memory, so the next query is one row read +
 //     the per-episode fixed part; each thread keeps only the visited bits it needs; capacity / current node are
 //     replicated scalars; the CVRP depot rule uses a register bitmask over demand ranks instead of a block-wide OR;
@@ -62,7 +67,10 @@ struct Smem {
   alignas(16) float part[8][32 * SPL];  // per-head share of every pointer logit: [head][node]
   alignas(16) float zbuf[2][32 * SPL];  // masked, temperature-scaled logits of the last two steps (deferred log-prob)
   alignas(16) uint2 red[4];             // per selection warp: (best key as order-preserving uint, node)
-  alignas(16) float lps[32];            // log-prob warp: lane partial sums of exp(z - Zb)
+  alignas(16) float lps[2][32];         // log-prob warps: lane partial sums of exp(z - Zb) of the last two steps
+  float lsel[2];                        // and z[a] - Zb of their chosen nodes
+  float ll;                             // ll warp, lane 0: the log-likelihood so far
+  float pen;                            // bookkeeping warp, lane 0: pctsp's saved penalties
   float dem[32 * SPL];                  // cvrp / sdvrp: demand; op: prize (node-indexed, depot 0)
   float lim[32 * SPL];                  // op: max_length per node (budget minus the way back); pctsp: penalty per node
   float2 loc[32 * SPL];
@@ -73,6 +81,22 @@ struct Smem {
   alignas(16) float wdyn[3 * E];              // [wk | wv | W_out^T wl]
   alignas(16) float pwk[32 * SPL * 8 + 8];    // ptab[n] . wk_h per (node, head); last 8 = the zero row
 };
+
+// Phase clocks, a diagnostic build only (-DCO_PHASE_CLOCKS, tools/rollout_phase_clocks.py): lane 0 of every warp
+// records clock64() at the top of each decode step, at arrival at / release from both block barriers, and at the top
+// of each instance, into co_phase_clk[b][dstep][warp][6] (slots: 0 step top, 1 B1 arrival, 2 B1 release, 3 B2
+// arrival, 4 B2 release, 5 instance top (dstep 0 row)).  Single-trajectory launches only; without the macro the
+// stamps compile to nothing.  The buffer must be set before the first launch: a constant-bank pointer with no null
+// test keeps the clock read off any load's latency.
+#ifdef CO_PHASE_CLOCKS
+static __constant__ unsigned long long* co_phase_clk;
+#define CO_PHASE_STAMP(row, slot)                                                                    \
+  do {                                                                                               \
+    if (lane == 0) co_phase_clk[(((size_t)b * T_max + (row)) * 8 + h) * 6 + (slot)] = clock64();   \
+  } while (0)
+#else
+#define CO_PHASE_STAMP(row, slot) do { } while (0)
+#endif
 
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -166,7 +190,10 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
   const bool forced_start = (S > 1) && (A.flags & CO_ROLLOUT_FORCED_START);
   const bool philox = (A.noise == nullptr);
   const bool sel_warp = h < NW;   // selection phase: thread tid < NS owns node nL = tid
-  const bool lp_warp = h == NW;   // the warp that computes the previous step's log-probability meanwhile
+  // warps that are idle between the two block barriers, and what they do there for the steps before
+  const bool lp_warp = h == NW;      // the exp partials of the previous step's log-probability
+  const bool bk_warp = h == NW + 1;  // the previous step's share of the reward and the outputs
+  const bool ll_warp = h == NW + 2;  // the sum, log and store of the log-probability of the step before that
   const int nL = sel_warp ? tid : NS - 1;
   const int nG = SPL * lane;      // first of this lane's SPL consecutive glimpse nodes
   const float clip = A.tanh_clipping, inv_temp = 1.0f / A.temperature;
@@ -176,6 +203,7 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
   float2 Kr[SPL][8], Vr[SPL][8], Lr[SPL][8];
 
   for (int b = blockIdx.x; b < B_inst; b += gridDim.x) {
+    CO_PHASE_STAMP(0, 5);
     __syncthreads();  // previous instance no longer reads shared memory
     const float* crow = A.cache + (size_t)b * N * CW;
     // ---- one HBM read of the instance: registers <- head slices of glimpse_key / glimpse_val / folded logit key
@@ -315,8 +343,8 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
 
     for (int s = 0; s < S; ++s) {
       const int traj = s * B_inst + b;  // start-major, rl4co/utils/ops.py:10-29
-      int64_t* act_row = A.actions_out + (size_t)traj * T_max;
-      float* lp_row = A.logp_out + (size_t)traj * T_max;
+      // output rows, addressed from the arguments at each store: no 64-bit row pointers are carried through the loop
+      const size_t row = (size_t)traj * T_max;
       // ---------------- reset (tsp/env.py:88-113, cvrp/env.py:98-124)
       // visited flags this thread needs: bit k = its glimpse node nG + k, bit 8 = its selection-phase node nL
       // (padding slots start as visited)
@@ -324,7 +352,9 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
 #pragma unroll
       for (int k = 0; k < SPL; ++k) mybits |= (nG + k >= N) ? (1u << k) : 0u;
       int cur = (ENV == CO_ENV_TSP) ? NS : 0;  // NS -> zero row: step-0 placeholder context
-      int prev = 0, first = 0, t = 0, dstep = 0, nvis = 0;
+      int first = 0, t = 0, dstep = 0, nvis = 0;
+      int prev = 0;      // bookkeeping warp: the last node it has accounted
+      float dist = 0.f;  // bookkeeping warp: the tour length (op: the collected prize)
       // cvrp: visited customers as a bitmask over demand RANKS (bits >= #customers pre-set), so the
       // unvisited customer of least demand is ffs(~mask): registers only, nothing shared is written
       uint32_t rmask[SPL];
@@ -333,7 +363,7 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
         const int lo = 32 * k, nc = N - 1;
         rmask[k] = (nc >= lo + 32) ? 0u : (nc <= lo ? 0xffffffffu : (0xffffffffu << (nc - lo)));
       }
-      float used = 0.f, dist = 0.f;
+      float used = 0.f;
       bool anyfeas = false, done = false, depot_seen = false;
       // (remaining) demand of this thread's glimpse nodes / selection node: constant for cvrp, dynamic for sdvrp
       float dmk[SPL], dL = dL0;
@@ -342,12 +372,12 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
       int nrem = 0;                 // sdvrp: customers with demand left
       int pend_a = -1;              // sdvrp: demand write-back deferred past the next barrier (see env_step)
       float pend_d = 0.f, FKW = 0.f;
-      float ll = 0.f;               // log-likelihood, accumulated by lane 0 of the log-prob warp
-      float pen = 0.f;              // pctsp: penalties of the visited customers (warp 0)
       // sdvrp serves demand in place (sm.dem): every further trajectory of the instance starts from the original demands
       // (every thread is past the previous trajectory's last read: the epilogue barrier)
       if (SD && s > 0 && tid < NS) sm.dem[tid] = (tid >= 1 && tid < N) ? A.demand[(size_t)b * (N - 1) + tid - 1] : 0.f;
       __syncthreads();  // previous trajectory finished with qfix
+      if (bk_warp && lane == 0) sm.pen = 0.f;
+      if (ll_warp && lane == 0) sm.ll = 0.f;
       if (tid < E) {
         float g = A.graph_ctx ? A.graph_ctx[(size_t)b * E + tid] : 0.f;
         if (ENV == CO_ENV_TSP && !forced_start) g += A.q_placeholder[tid];
@@ -361,23 +391,16 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
           mybits |= (dd < (unsigned)SPL) ? (1u << dd) : 0u;
           mybits |= (a == nL) ? 0x100u : 0u;
         }
-        if (!OP && h == 0) {  // incremental tour length: warp 0 only (thread 0 writes the reward)
-          const float2 pa = sm.loc[a], pp = sm.loc[prev];
-          const float dx = pa.x - pp.x, dy = pa.y - pp.y;
-          if (VRP || t != 0) dist += sqrtf(dx * dx + dy * dy);
-        }
         if (ENV == CO_ENV_TSP) {
           if (t == 0) first = a;
         } else if (OP) {
           // op/env.py:72-105: the tour length feeds the mask and the context (every thread replays it, `used`); the
-          // collected prize is the reward (`dist`, warp 0); the depot re-entered after step 0 ends the episode
-          used = used + dist2_fma(sm.loc[a], sm.loc[prev]);
-          if (h == 0) dist += sm.dem[a];
+          // collected prize is the reward (see account); the depot re-entered after step 0 ends the episode
+          used = used + dist2_fma(sm.loc[a], sm.loc[cur]);
           depot_seen = depot_seen || (a == 0);
         } else if (PC) {
-          // pctsp/env.py:62-93: collected prize (replicated: depot rule + context), saved penalties (warp 0, reward)
+          // pctsp/env.py:62-93: collected prize (replicated: depot rule + context); saved penalties: see account
           used = used + sm.dem[a];
-          if (h == 0) pen += sm.lim[a];
           nvis += (a != 0) ? 1 : 0;
           depot_seen = depot_seen || (a == 0);
         } else if (SD) {
@@ -414,34 +437,52 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
           }
           anyfeas = (pmin < N - 1) && !((sm.dem[sm.order[pmin < N - 1 ? pmin : 0]] + used) > thr);
         }
-        prev = a; cur = a; ++t;
+        cur = a; ++t;
         // cvrp: all nodes incl. the depot visited; sdvrp: no positive demand left (sdvrp/env.py:71)
         done = (ENV == CO_ENV_TSP) ? (t >= N) : ((OP || PC) ? (a == 0 && t > 1) : (SD ? (nrem == 0) : (nvis >= N)));
       };
-      // log-softmax(z)[a] of one finished step from its z row (log-prob warp; decoding.py:188,352-356): exact
-      // exp-sum with the fixed offset Zb; masked nodes hold -inf -> 2^-inf = 0
-      auto logp_of = [&](int buf, int a_sel, int t_out) {
+      // log-softmax(z)[a] of a finished step (decoding.py:188,352-356): exact exp-sum with the fixed offset Zb; masked
+      // nodes hold -inf -> 2^-inf = 0.  First half (lp warp): the lane partials from the step's z row, whose chosen
+      // node is cur; second half (ll warp, one step later): their sum, log and store.
+      auto logp_partials = [&](int buf) {
         const float* zb = sm.zbuf[buf];
         float sacc = 0.f;
 #pragma unroll
         for (int k = 0; k < SPL; ++k) sacc += ex2((zb[nG + k] - Zb) * LOG2E);
+        sm.lps[buf][lane] = sacc;
+        if (lane == 0) sm.lsel[buf] = zb[cur] - Zb;
+      };
+      auto logp_finish = [&](int buf, int t_out) {
         // 32 lane partials -> every lane adds all of them in a fixed tree from shared memory (shorter dependent
         // chain than five shuffles; this warp must finish inside the other warps' selection phase)
-        sm.lps[lane] = sacc;
-        __syncwarp();
-        const float4* lq = reinterpret_cast<const float4*>(sm.lps);
+        const float ll_prev = sm.ll;  // read with the partials, not after the tree
+        const float4* lq = reinterpret_cast<const float4*>(sm.lps[buf]);
         const float4 q0 = lq[0], q1 = lq[1], q2 = lq[2], q3 = lq[3], q4 = lq[4], q5 = lq[5], q6 = lq[6], q7 = lq[7];
         const float t0 = ((q0.x + q0.y) + (q0.z + q0.w)) + ((q1.x + q1.y) + (q1.z + q1.w));
         const float t1 = ((q2.x + q2.y) + (q2.z + q2.w)) + ((q3.x + q3.y) + (q3.z + q3.w));
         const float t2 = ((q4.x + q4.y) + (q4.z + q4.w)) + ((q5.x + q5.y) + (q5.z + q5.w));
         const float t3 = ((q6.x + q6.y) + (q6.z + q6.w)) + ((q7.x + q7.y) + (q7.z + q7.w));
-        sacc = (t0 + t1) + (t2 + t3);
-        __syncwarp();  // lps is rewritten by the next call
-        const float lp = (zb[a_sel] - Zb) - lg2(sacc) * LN2;
+        const float sacc = (t0 + t1) + (t2 + t3);
+        const float lp = sm.lsel[buf] - lg2(sacc) * LN2;
         if (lane == 0) {
-          lp_row[t_out] = lp;
-          ll += lp;
+          sm.ll = ll_prev + lp;
+          A.logp_out[row + t_out] = lp;
         }
+      };
+      // per-step work that only the reward and the outputs need (bookkeeping warp, one step behind): the tour length,
+      // op's prize, pctsp's saved penalties, the action store.  The tour length is the longest chain between the
+      // barriers, so it goes first and without a branch: tsp's first step adds +0.0f to dist = +0, exactly as skipping.
+      auto account = [&](int a, int ta) {
+        if (!OP) {
+          const float2 pa = sm.loc[a], pp = sm.loc[prev];
+          const float dx = pa.x - pp.x, dy = pa.y - pp.y;
+          const float leg = sqrtf(dx * dx + dy * dy);
+          dist += (VRP || ta != 0) ? leg : 0.f;
+        }
+        if (OP) dist += sm.dem[a];
+        if (PC && lane == 0) sm.pen += sm.lim[a];
+        if (lane == 0) A.actions_out[row + ta] = a;
+        prev = a;
       };
 
       if (SD) {  // customers with demand: counted by every thread from shared memory (uniform)
@@ -451,8 +492,9 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
       }
       if (forced_start) {  // multistart pre_decoder_hook, decoding.py:309-326 + ops.py:128-149
         const int a0 = (s % A.num_loc) + (VRP ? 1 : 0);
-        if (tid == 0) { act_row[0] = a0; lp_row[0] = 0.f; }
+        if (tid == 0) A.logp_out[row] = 0.f;
         env_step(a0);
+        if (bk_warp) account(a0, 0);
         if (ENV == CO_ENV_TSP) {
           __syncthreads();  // qfix initialised
           add_first(a0);
@@ -468,6 +510,7 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
       }
 
       while (!done && t < T_max) {
+        CO_PHASE_STAMP(dstep, 0);
         // early, latency-tolerant loads for this step
         int forced = 0;
         float gum = 0.f;  // -log q, q ~ Exp(1): Gumbel perturbation for sampling
@@ -578,7 +621,9 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
           else if (SPL == 2) *reinterpret_cast<float2*>(pdst) = make_float2(pl[0], pl[SPL > 1 ? 1 : 0]);
           else *pdst = pl[0];
         }
+        CO_PHASE_STAMP(dstep, 1);
         __syncthreads();  // B1: every head's share of every logit is in shared memory
+        CO_PHASE_STAMP(dstep, 2);
 
         if (SD && tid == 0 && pend_a >= 0) sm.dem[pend_a] = pend_d;  // deferred demand write-back (every thread is
                                                                      // past the env_step that read the old value)
@@ -599,10 +644,16 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
             const unsigned vote = __ballot_sync(FULL, key == wkey);
             if (lane == 0) sm.red[h] = make_uint2(wkey, (unsigned)(32 * h + __ffs(vote) - 1));  // lowest node wins ties
           }
+        } else if (bk_warp) {  // longest chain first; then the earlier steps' log-probabilities, off the critical path
+          if (dstep > 0) account(cur, t - 1);
+        } else if (ll_warp) {
+          if (dstep > 1) logp_finish(dstep & 1, t - 2);
         } else if (lp_warp && dstep > 0) {
-          logp_of((dstep - 1) & 1, prev, t - 1);  // the previous step's log-probability, off the critical path
+          logp_partials((dstep - 1) & 1);
         }
+        CO_PHASE_STAMP(dstep, 3);
         __syncthreads();  // B2: per-warp winners complete
+        CO_PHASE_STAMP(dstep, 4);
         int a;
         if (MODE == CO_MODE_EVALUATE) {
           a = (forced < 0 || forced >= N) ? 0 : forced;
@@ -618,7 +669,6 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
           const unsigned kb = b23 ? r1.z : r1.x, ib = b23 ? r1.w : r1.y;
           a = (int)((kb > ka) ? ib : ia);
         }
-        if (tid == 0) act_row[t] = a;
 
         // ---------------- environment step
         const bool was_first = (ENV == CO_ENV_TSP) && (t == 0);
@@ -635,18 +685,21 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
 
       // ---------------- epilogue: last log-probability, reward, log-likelihood, padding
       __syncthreads();
-      if (lp_warp) {
-        if (dstep > 0) logp_of((dstep - 1) & 1, prev, t - 1);
-        if (lane == 0) A.loglik_out[traj] = ll;
+      if (lp_warp && dstep > 0) logp_partials((dstep - 1) & 1);
+      __syncthreads();  // the last step's partials are in shared memory
+      if (ll_warp) {  // the last two steps (decode step k has the output index t - dstep + k)
+        for (int k = dstep > 1 ? dstep - 2 : 0; k < dstep; ++k) logp_finish(k & 1, t - dstep + k);
+        if (lane == 0) A.loglik_out[traj] = sm.ll;
       }
-      if (tid == 0) {
+      if (bk_warp && dstep > 0) account(cur, t - 1);
+      if (bk_warp && lane == 0) {
         const float2 pa = sm.loc[(ENV == CO_ENV_TSP) ? first : 0], pp = sm.loc[prev];
         const float dx = pa.x - pp.x, dy = pa.y - pp.y;
         float rw = OP ? dist : -(dist + sqrtf(dx * dx + dy * dy));  // op: the collected prize
         if (PC) {  // pctsp/env.py:153-172: saved penalties - (length + all penalties)
           float total = 0.f;
           for (int n = 1; n < N; ++n) total += sm.lim[n];
-          rw = pen - (-rw + total);
+          rw = sm.pen - (-rw + total);
         }
         A.reward_out[traj] = rw;
         if (A.steps_out) A.steps_out[traj] = t;
@@ -654,7 +707,7 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
         if (A.max_steps_out) atomicMax(A.max_steps_out, t);
       }
       // done instances keep selecting the depot with log-prob 0 until the batch finishes
-      for (int c = t + tid; c < T_max; c += 256) { act_row[c] = 0; lp_row[c] = 0.f; }
+      for (int c = t + tid; c < T_max; c += 256) { A.actions_out[row + c] = 0; A.logp_out[row + c] = 0.f; }
     }
   }
 }

@@ -107,13 +107,15 @@ def _nvcc() -> str:
     return nvcc if os.path.exists(nvcc) else "nvcc"
 
 
-def build(force: bool = False, verbose: bool = False, extra_flags: list[str] | None = None) -> str:
+def build(force: bool = False, verbose: bool = False, extra_flags: list[str] | None = None,
+          lib_path: str = LIB_PATH) -> str:
     """Compile libcorollout.so in-tree for sm_90a (nvcc cross-compiles without a GPU).
-    Translation units are compiled in parallel, then linked."""
+    Translation units are compiled in parallel, then linked.  A diagnostic variant (`extra_flags`) goes to its own
+    `lib_path`, with its objects beside it."""
     deps = [os.path.join(CSRC, s) for s in SOURCES + HEADERS] + [os.path.join(INCLUDE, "corollout.h")]
-    if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(s) for s in deps):
-        return LIB_PATH
-    objdir = os.path.join(_HERE, "build")
+    if not force and os.path.exists(lib_path) and all(os.path.getmtime(lib_path) >= os.path.getmtime(s) for s in deps):
+        return lib_path
+    objdir = os.path.join(os.path.dirname(os.path.abspath(lib_path)), "build")
     os.makedirs(objdir, exist_ok=True)
     procs = []
     for s in SOURCES:
@@ -129,12 +131,12 @@ def build(force: bool = False, verbose: bool = False, extra_flags: list[str] | N
         if p.returncode != 0:
             raise NativeLibraryError(f"nvcc failed on {s} ({p.returncode}):\n{out}")
         objs.append(obj)
-    link = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB_PATH] + objs
+    link = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", lib_path] + objs
     res = subprocess.run(link, capture_output=True, text=True)
     if res.returncode != 0:
         raise NativeLibraryError(f"link failed ({res.returncode}):\n{res.stdout}\n{res.stderr}")
     build.last_log = "\n".join(log)
-    return LIB_PATH
+    return lib_path
 
 
 _lib = None
