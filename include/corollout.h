@@ -190,17 +190,16 @@ int co_cvrp_local_search(const float* locs, const float* dist, const float* dema
 
 /* Weights of the decoder path, device pointers, all float32, no biases
  * (rl4co/models/zoo/am/policy.py:65,70).  *_t tensors are TRANSPOSED copies
- * ([in, out] row-major) prepared once per weight update by the host side. */
+ * ([in, out] row-major) prepared once per weight update by the host side.
+ * pointer.project_out is not among them: it is folded into logit_key (see co_pointer_logits). */
 typedef struct co_decoder_weights {
   const float* project_context_t; /* [ctx_dim, E]; ctx_dim = 2E (tsp) or E+1 (cvrp)   */
   const float* w_placeholder;     /* [2E] (tsp only, else NULL)                       */
-  const float* project_out_t;     /* [E, E] transposed pointer.project_out.weight, or  */
-                                  /* NULL when logit_key is pre-multiplied by it       */
   /* dynamic embedding (sdvrp: SDVRPDynamicEmbedding, nn/env_embeddings/dynamic.py:60-78; am/decoder.py:142-154):
    * glimpse_key / glimpse_val / logit_key of node n get + dynamic_feature[j, n] * dynamic_w[0:E | E:2E | 2E:3E].
    * Both NULL for static embeddings (tsp, cvrp). */
-  const float* dynamic_w;         /* [3E] = projection.weight[:, 0]; the logit third folded with project_out   */
-                                  /* (W_out^T w_l) when project_out_t == NULL                                   */
+  const float* dynamic_w;         /* [3E] = projection.weight[:, 0], the logit third folded with project_out    */
+                                  /* (W_out^T w_l)                                                              */
   const float* dynamic_feature;   /* [B_traj, N] per-step node feature (sdvrp: remaining demand, depot = 0)     */
 } co_decoder_weights;
 
@@ -213,8 +212,8 @@ typedef struct co_decoder_weights {
  *   cvrp: current_node [B_traj] int64, used_capacity / vehicle_capacity [B_traj] f32
  * glimpse_key / glimpse_val / logit_key rows are `ld` floats apart (ld = E for the
  * reference's contiguous tensors, or the fused-cache row width for views into it; 0 = E).
- * w->project_out_t == NULL means logit_key already holds the folded rows
- * logit_key @ project_out.weight (block 2 of the rollout cache) and the projection is skipped. */
+ * logit_key holds the folded rows logit_key @ project_out.weight (block 2 of the rollout cache),
+ * so the glimpse is the concatenated head output itself. */
 int co_pointer_logits(int env_kind, const co_decoder_weights* w, const float* node_emb,
                       const float* graph_ctx /* [B_inst,E] or NULL */,
                       const float* glimpse_key, const float* glimpse_val,
@@ -248,11 +247,10 @@ int co_select_action(const float* logits, const uint8_t* action_mask, const floa
  * The cache is the layout written by FusedAttentionModelDecoder._precompute_cache:
  *   cache[B_inst][N][co_cache_width(env_kind)] float32, column blocks of E floats:
  *     0: glimpse_key   1: glimpse_val   2: logit_key @ project_out (folded)
- *     3: node_emb @ Wctx[:, :E]^T  (tsp: "first node" table; cvrp: current-node table)
+ *     3: node_emb @ Wctx[:, :E]^T  (tsp: "first node" table; other envs: current-node table)
  *     4: node_emb @ Wctx[:, E:2E]^T (tsp only: current-node table)
  */
 #define CO_ROLLOUT_FORCED_START 1 /* S>1: first action of start s is forced (multistart) */
-#define CO_ROLLOUT_NO_PREFETCH 2  /* diagnostic: do not prefetch the next instance's cache rows into L2 */
 
 typedef struct co_rollout_args {
   int32_t env_kind;     /* CO_ENV_*                                                    */
@@ -283,13 +281,9 @@ typedef struct co_rollout_args {
   int32_t* steps_out;        /* [B_traj]  decode steps until done (incl. forced start) */
   int32_t* max_steps_out;    /* [1] device int32, caller-zeroed: max over trajectories */
   float* used_capacity_out;  /* [B_traj] final used capacity (cvrp) or NULL            */
-  /* narrow tsp cache (no first-node table) -- the first-node half of project_context
-   * (context.py:129-133) becomes one 128x128 GEMV per episode inside the kernel            */
-  const float* node_emb;     /* [B_inst, N, E] encoder output; tsp with cache_width 4E  */
-  const float* w_first;      /* [E, E] = project_context.weight[:, :E] row-major; same   */
-  int32_t cache_width;       /* floats per row of `cache`: 4E, or 5E = tsp layout with   */
-                             /* the first-node table; 0 = co_cache_width(env_kind)       */
-  int32_t reserved0;
+  int32_t cache_width;       /* floats per row of `cache`, must equal                   */
+                             /* co_cache_width(env_kind); 0 = that width                 */
+  int32_t reserved0;         /* keeps the pointers below 8-byte aligned                  */
   /* sdvrp: dynamic-embedding weights [wk | wv | W_out^T wl] = SDVRPDynamicEmbedding.projection.weight[:, 0] with
    * the logit third folded like block 2 of the cache (nn/env_embeddings/dynamic.py:60-78); NULL otherwise */
   const float* dyn_w;        /* [3E] */
@@ -317,7 +311,7 @@ typedef struct co_rollout_args {
  *   A row whose column 0 is out of range, that takes an action the replayed mask forbids (or outside [0, N)), or that
  *   is not done within min(T, 2 * 32 * ceil(N / 32)) columns contributes nothing, gets loglik = NaN and adds 1 to
  *   *bad_rows (device int32, caller-zeroed, nullable).
- *   cache: tsp the 5E layout (first-node table; the 4E layout is CO_ERR_UNSUPPORTED), cvrp 4E; 16-byte aligned.
+ *   cache: tsp the 5E layout (first-node table; another width is CO_ERR_UNSUPPORTED), cvrp 4E; 16-byte aligned.
  *   Errors: env other than tsp / cvrp, N > co_rollout_max_nodes() or tanh_clipping <= 0: CO_ERR_UNSUPPORTED; null
  *   pointers, B_inst < 0, N < 2, num_rows < 1, T < 1 (tsp: T < N), temperature <= 0, a wrong cvrp cache width,
  *   missing cvrp demand / w_capacity or misaligned cache / dLf: CO_ERR_BAD_ARG. */
@@ -343,7 +337,7 @@ typedef struct co_eas_grad_args {
 } co_eas_grad_args;
 int co_eas_key_grad(const co_eas_grad_args* args, void* stream);
 
-int co_cache_width(int env_kind); /* floats per node row of the widest rollout cache layout (tsp 5E, cvrp 4E) */
+int co_cache_width(int env_kind); /* floats per node row of the rollout cache (tsp 5E, the other envs 4E) */
 /* largest N the persistent kernel is instantiated for (else CO_ERR_UNSUPPORTED) */
 int co_rollout_max_nodes(void);
 int co_rollout(const co_rollout_args* args, void* stream);

@@ -12,8 +12,8 @@ namespace co {
 // one CTA (128 threads = 4 warps) per trajectory
 template <int ENV>
 __global__ void __launch_bounds__(128) pointer_logits_kernel(
-    const float* __restrict__ wctx_t, const float* __restrict__ w_placeholder, const float* __restrict__ wout_t,
-    const float* __restrict__ node_emb, const float* __restrict__ graph_ctx, const float* __restrict__ Kc,
+    const float* __restrict__ wctx_t, const float* __restrict__ w_placeholder, const float* __restrict__ node_emb,
+    const float* __restrict__ graph_ctx, const float* __restrict__ Kc,
     const float* __restrict__ Vc, const float* __restrict__ Lc, const uint8_t* __restrict__ mask,
     const int64_t* __restrict__ first_node, const int64_t* __restrict__ current_node,
     const int64_t* __restrict__ istep, const float* __restrict__ used, const float* __restrict__ cap,
@@ -22,9 +22,8 @@ __global__ void __launch_bounds__(128) pointer_logits_kernel(
   extern __shared__ float sm[];
   float* ctx = sm;             // [2E] context input
   float* q = ctx + 2 * E;      // [E]
-  float* o = q + E;            // [E] concatenated heads
-  float* g2 = o + E;           // [E] glimpse after project_out
-  float* sc = g2 + E;          // [H][N] scores -> attention weights
+  float* o = q + E;            // [E] concatenated heads = glimpse (logit_key is folded with project_out)
+  float* sc = o + E;           // [H][N] scores -> attention weights
 
   const int j = blockIdx.x;
   const int b = j % B_inst;
@@ -103,18 +102,8 @@ __global__ void __launch_bounds__(128) pointer_logits_kernel(
     o[t] = acc;
   }
   __syncthreads();
-  {  // glimpse = project_out(o); wout_t == NULL means logit_key is already folded (L @ W_out)
-    float acc = 0.f;
-    if (wout_t) {
-      for (int k = 0; k < E; ++k) acc = fmaf(o[k], wout_t[(size_t)k * E + t], acc);
-    } else {
-      acc = o[t];
-    }
-    g2[t] = acc;
-  }
-  __syncthreads();
   {  // logits[n] = glimpse . L[n] / sqrt(E)
-    const float4 gv = reinterpret_cast<const float4*>(g2)[lane];
+    const float4 gv = reinterpret_cast<const float4*>(o)[lane];
     float4 wl = make_float4(0.f, 0.f, 0.f, 0.f);
     if (frow) wl = reinterpret_cast<const float4*>(dyn_w + 2 * E)[lane];
     for (int n = w; n < N; n += 4) {
@@ -201,7 +190,7 @@ extern "C" int co_pointer_logits(int env_kind, const co_decoder_weights* w, cons
   if (B_traj < 0 || B_inst <= 0 || N <= 0 || (B_traj % B_inst) != 0)
     return fail(CO_ERR_BAD_ARG, "co_pointer_logits: bad shape%s B_traj=%lld B_inst=%lld", "", B_traj, B_inst);
   if (B_traj == 0) return CO_OK;
-  size_t smem = (size_t)(5 * E + H * N) * sizeof(float);
+  size_t smem = (size_t)(4 * E + H * N) * sizeof(float);
   if (smem > 200 * 1024) return fail(CO_ERR_UNSUPPORTED, "co_pointer_logits: N too large%s (%lld)", "", N);
   cudaStream_t st = (cudaStream_t)stream;
   if (env_kind == CO_ENV_TSP) {
@@ -213,7 +202,7 @@ extern "C" int co_pointer_logits(int env_kind, const co_decoder_weights* w, cons
       attr = true;
     }
     pointer_logits_kernel<CO_ENV_TSP><<<B_traj, 128, smem, st>>>(
-        w->project_context_t, w->w_placeholder, w->project_out_t, node_emb, graph_ctx, glimpse_key, glimpse_val,
+        w->project_context_t, w->w_placeholder, node_emb, graph_ctx, glimpse_key, glimpse_val,
         logit_key, action_mask, first_node, current_node, i, nullptr, nullptr, nullptr, nullptr, logits_out, B_inst, N, ld);
   } else if (env_kind == CO_ENV_CVRP || env_kind == CO_ENV_SDVRP) {  // both use VRPContext (context.py:26,137-149)
     if ((w->dynamic_w == nullptr) != (w->dynamic_feature == nullptr))
@@ -227,7 +216,7 @@ extern "C" int co_pointer_logits(int env_kind, const co_decoder_weights* w, cons
       attr = true;
     }
     pointer_logits_kernel<CO_ENV_CVRP><<<B_traj, 128, smem, st>>>(
-        w->project_context_t, nullptr, w->project_out_t, node_emb, graph_ctx, glimpse_key, glimpse_val, logit_key,
+        w->project_context_t, nullptr, node_emb, graph_ctx, glimpse_key, glimpse_val, logit_key,
         action_mask, nullptr, current_node, nullptr, used_capacity, vehicle_capacity, w->dynamic_w, w->dynamic_feature,
         logits_out, B_inst, N, ld);
   } else {

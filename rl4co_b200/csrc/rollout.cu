@@ -1,7 +1,5 @@
 // C-ABI entry of the persistent rollout (argument validation + dispatch); kernels live in
 // rollout_impl.cuh, instantiated in rollout_tsp.cu / rollout_cvrp.cu.
-#include <stdlib.h>
-
 #include "co_common.cuh"
 
 namespace co {
@@ -40,19 +38,14 @@ extern "C" int co_rollout(const co_rollout_args* args, void* stream) {
   if ((A.flags & CO_ROLLOUT_FORCED_START) && A.num_loc < 1) return fail(CO_ERR_BAD_ARG, "co_rollout: num_loc required for forced starts%s");
   if (A.B_inst == 0) return CO_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  // S > 1 trajectories per instance: the query-batched kernel advances 4 of them per pass
-  static const bool use_ms = !(getenv("CO_ROLLOUT_MS") && atoi(getenv("CO_ROLLOUT_MS")) == 0);
-  const bool ms = use_ms && A.num_starts > 1;
+  // S > 1 trajectories per instance: tsp and cvrp run the query-batched kernel, which advances 4 of them per pass, so
+  // they never reach the single-trajectory kernel with S > 1
+  const bool ms = A.num_starts > 1;
   if (A.cache_width == 0) A.cache_width = co_cache_width(A.env_kind);
-  if (getenv("CO_ROLLOUT_PREFETCH") && atoi(getenv("CO_ROLLOUT_PREFETCH")) == 0) A.flags |= CO_ROLLOUT_NO_PREFETCH;
   if (A.env_kind == CO_ENV_TSP) {
     if (!A.q_placeholder) return fail(CO_ERR_BAD_ARG, "co_rollout: q_placeholder required for tsp%s");
     if (A.T_max < A.N) return fail(CO_ERR_BAD_ARG, "co_rollout: T_max < N%s");
-    if (A.cache_width != 4 * E && A.cache_width != 5 * E) return fail(CO_ERR_BAD_ARG, "co_rollout: tsp cache_width must be 4E or 5E%s");
-    if (A.cache_width == 4 * E && (!A.node_emb || !A.w_first))
-      return fail(CO_ERR_BAD_ARG, "co_rollout: tsp cache_width 4E needs node_emb and w_first%s");
-    if (ms && A.cache_width != 5 * E)
-      return fail(CO_ERR_UNSUPPORTED, "co_rollout: the multistart kernel needs the 5E tsp cache (first-node table)%s");
+    if (A.cache_width != 5 * E) return fail(CO_ERR_BAD_ARG, "co_rollout: tsp cache_width must be 5E%s");
     return ms ? rollout_ms_tsp(A, st) : rollout_tsp(A, st);
   }
   if (A.env_kind == CO_ENV_CVRP) {

@@ -35,9 +35,8 @@
 //   * exactly two block barriers per node selection; no state in HBM.
 // HBM traffic per instance = one read of its cache rows + T*(8+4) B of outputs.
 //
-// Cache layouts (args.cache_width): 4E = [K | V | L' | cur-table]: the TSP first-node half of the context
-// projection is one 128x128 GEMV per episode from node_emb / w_first;  5E (tsp default) = [K | V | L' | first-table |
-// cur-table] (the multistart kernel reads one table row per start).
+// Cache layout, one per env: tsp 5E = [K | V | L' | first-table | cur-table], so the first-node half of the context
+// projection is one table-row read per episode; the other envs 4E = [K | V | L' | cur-table].
 #pragma once
 #include "co_common.cuh"
 
@@ -61,7 +60,6 @@ struct Smem {
   float ptab[(32 * SPL + 1) * E];       // current-node context table; last row = zeros
   float qfix[E];                        // per-episode fixed part of the query
   float wcap[E];                        // cvrp: remaining-capacity column of project_context
-  float hfirst[E];                      // tsp, 4E cache: embedding of the first node (GEMV operand; 16-byte aligned)
   float tile[8][32 * TILE_LD];          // per-warp transpose tile for the value reduction
   alignas(16) float oh[8][D];           // per-warp broadcast of the un-normalised head output
   alignas(16) float part[8][32 * SPL];  // per-head share of every pointer logit: [head][node]
@@ -130,25 +128,6 @@ __device__ __forceinline__ float warp_sum_fixed(float x) {
   return fmaf((float)Ls, 1.0f / (S * S), (float)Hs * (1.0f / S));
 }
 
-// tsp, 4E cache: qfix[e] += sum_c w_first[e][c] * hfirst[c]  (project_context[:, :E] @ h[first], context.py:129-133).
-// Once per episode; kept out of line so that its address arithmetic does not cost the episode loop registers.
-// 256 threads: two per output channel, 64 input channels each.
-static __device__ __noinline__ void first_node_gemv(const float* __restrict__ w_first, const float* hfirst, float* qfix, int tid) {
-  const int e = tid >> 1, half = tid & 1;
-  const float4* wr = reinterpret_cast<const float4*>(w_first + (size_t)e * E + 64 * half);
-  const float4* hv = reinterpret_cast<const float4*>(hfirst + 64 * half);
-  float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-  for (int c = 0; c < 16; c += 2) {
-    const float4 w0 = __ldg(wr + c), x0 = hv[c], w1 = __ldg(wr + c + 1), x1 = hv[c + 1];
-    s0 = fmaf(w0.x, x0.x, s0); s0 = fmaf(w0.y, x0.y, s0); s0 = fmaf(w0.z, x0.z, s0); s0 = fmaf(w0.w, x0.w, s0);
-    s1 = fmaf(w1.x, x1.x, s1); s1 = fmaf(w1.y, x1.y, s1); s1 = fmaf(w1.z, x1.z, s1); s1 = fmaf(w1.w, x1.w, s1);
-  }
-  float sacc = s0 + s1;
-  sacc += __shfl_xor_sync(FULL, sacc, 1);
-  if (half == 0) qfix[e] += sacc;
-}
-
 // 2-norm of a coordinate difference as torch's CPU reduction rounds it (op_kernels.cu): sqrt(fma(dy, dy, dx * dx))
 __device__ __forceinline__ float dist2_fma(float2 a, float2 b) {
   const float dx = a.x - b.x, dy = a.y - b.y;
@@ -169,13 +148,12 @@ __device__ __forceinline__ bool feasible(int n, bool visbit, float d, float used
   return !visbit && !((d + used) > thr);
 }
 
-template <int SPL, int ENV, int MODE, int CWB>  // CWB = cache blocks of E floats per node row: 4, or 5 (tsp first-node table)
+template <int SPL, int ENV, int MODE>
 __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_rollout_args A) {
   using C = Cfg<SPL>;
   constexpr int NS = C::NS, NW = C::NW;
-  constexpr int CW = CWB * E;        // cache row width: 4E, or 5E (tsp with the first-node table)
-  constexpr int CUR_BLK = CWB - 1;   // block holding the current-node table (always the last one)
-  constexpr bool first_table = (ENV == CO_ENV_TSP) && (CWB == 5);
+  constexpr int CW = (ENV == CO_ENV_TSP ? 5 : 4) * E;  // cache row width (tsp: with the first-node table)
+  constexpr int CUR_BLK = (ENV == CO_ENV_TSP ? 4 : 3);  // block holding the current-node table (always the last one)
   constexpr bool VRP = (ENV != CO_ENV_TSP);        // depot env with capacity context (cvrp, sdvrp)
   constexpr bool SD = (ENV == CO_ENV_SDVRP);       // split deliveries: dynamic demand + dynamic embedding
   constexpr bool OP = (ENV == CO_ENV_OP);          // orienteering: `used` is the tour length, `cap` the budget at the depot
@@ -309,15 +287,10 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
 #pragma unroll
       for (int k = 0; k < SPL; ++k) out[k] = a2[k].x + a2[k].y;
     };
-    // tsp: qfix += project_context[:, :E] @ h[first] (context.py:129-133); callers barrier before and after
+    // tsp: qfix += project_context[:, :E] @ h[first] (context.py:129-133), the first-node table row; callers barrier
+    // before and after
     auto add_first = [&](int a_first) {
-      if (first_table) {
-        if (tid < E) sm.qfix[tid] += __ldg(crow + (size_t)a_first * CW + 3 * E + tid);
-      } else {
-        if (tid < E) sm.hfirst[tid] = __ldg(A.node_emb + ((size_t)b * N + a_first) * E + tid);
-        __syncthreads();
-        first_node_gemv(A.w_first, sm.hfirst, sm.qfix, tid);
-      }
+      if (tid < E) sm.qfix[tid] += __ldg(crow + (size_t)a_first * CW + 3 * E + tid);
     };
     float WK[SPL], FK[SPL];
 #pragma unroll
@@ -330,7 +303,7 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
       for (int c = 0; c < D; ++c) WKW = fmaf(sm.wcap[h * D + c], sm.wdyn[h * D + c], WKW);  // wcap_h . wk_h
       wv_d = sm.wdyn[E + h * D + (lane & 15)];
     }
-    if (!(A.flags & CO_ROLLOUT_NO_PREFETCH) && b + (int)gridDim.x < B_inst) {  // next instance's cache rows -> L2
+    if (b + (int)gridDim.x < B_inst) {  // next instance's cache rows -> L2
       // only the four blocks the kernel reads (K, V, L', current-node table): with the 5E layout the first-node table
       // block would otherwise be pulled from HBM for nothing
       const char* nxt = reinterpret_cast<const char*>(A.cache + (size_t)(b + gridDim.x) * N * CW);
@@ -490,15 +463,11 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
         anyfeas = (nrem > 0) && !(used >= cap);
         done = (nrem == 0);
       }
-      if (forced_start) {  // multistart pre_decoder_hook, decoding.py:309-326 + ops.py:128-149
+      if (forced_start) {  // multistart pre_decoder_hook, decoding.py:309-326 + ops.py:128-149 (sdvrp, op, pctsp)
         const int a0 = (s % A.num_loc) + (VRP ? 1 : 0);
         if (tid == 0) A.logp_out[row] = 0.f;
         env_step(a0);
         if (bk_warp) account(a0, 0);
-        if (ENV == CO_ENV_TSP) {
-          __syncthreads();  // qfix initialised
-          add_first(a0);
-        }
       } else if (ENV == CO_ENV_CVRP) {
         anyfeas = !((sm.dem[sm.order[0]] + used) > thr);
       }
@@ -712,9 +681,9 @@ __global__ void __launch_bounds__(256, Cfg<SPL>::MINB) rollout_kernel(const co_r
   }
 }
 
-template <int SPL, int ENV, int MODE, int CWB>
+template <int SPL, int ENV, int MODE>
 static int launch(const co_rollout_args& A, cudaStream_t st) {
-  auto kern = rollout_kernel<SPL, ENV, MODE, CWB>;
+  auto kern = rollout_kernel<SPL, ENV, MODE>;
   const size_t smem = sizeof(Smem<SPL>);
   static PerDeviceOnce once;
   static int ctas_per_sm = 1;
@@ -737,12 +706,8 @@ static int dispatch(const co_rollout_args& A, cudaStream_t st) {
   const int spl = A.N <= 32 ? 1 : (A.N <= 64 ? 2 : 4);
   const int mode = A.select_mode == CO_SELECT_GREEDY ? CO_MODE_GREEDY
                    : (A.select_mode == CO_SELECT_EVALUATE ? CO_MODE_EVALUATE : CO_MODE_SAMPLE);
-  const int cwb = A.cache_width / E;
-#define CO_CASE(S_, M_)                                                                      \
-  if (spl == S_ && mode == M_) {                                                             \
-    if (cwb == 4) return launch<S_, ENV, M_, 4>(A, st);                                      \
-    if (ENV == CO_ENV_TSP && cwb == 5) return launch<S_, ENV, M_, (ENV == CO_ENV_TSP ? 5 : 4)>(A, st); \
-  }
+#define CO_CASE(S_, M_) \
+  if (spl == S_ && mode == M_) return launch<S_, ENV, M_>(A, st);
   CO_CASE(1, CO_MODE_GREEDY) CO_CASE(2, CO_MODE_GREEDY) CO_CASE(4, CO_MODE_GREEDY)
   CO_CASE(1, CO_MODE_SAMPLE) CO_CASE(2, CO_MODE_SAMPLE) CO_CASE(4, CO_MODE_SAMPLE)
   CO_CASE(1, CO_MODE_EVALUATE) CO_CASE(2, CO_MODE_EVALUATE) CO_CASE(4, CO_MODE_EVALUATE)

@@ -12,14 +12,11 @@ What differs is the cache layout.  ``_precompute_cache`` does ONE GEMM
     2  logit_key @ project_out.weight  (rows 2E:3E, folded with pointer.project_out so the
                                         per-step 128x128 projection disappears:
                                         logits = heads . (L W_out)[n] == (W_out heads) . L[n])
-    [3 embeddings @ Wctx[:, :E]^T      tsp, `first_table=True` (default): first-node half of
-                                        project_context as a table -- the multistart kernel reads one
-                                        row per start, a single-start episode one row.  `first_table=
-                                        False` (CO_TSP_FIRST_TABLE=0) leaves the block out and the
-                                        kernel does one 128x128 GEMV per episode instead: 20 % less GEMM
-                                        output for more work in the rollout kernel]
+    [3 embeddings @ Wctx[:, :E]^T      tsp only: first-node half of project_context as a table --
+                                        the multistart kernel reads one row per start, a single-start
+                                        episode one row]
     last  embeddings @ Wctx_cur^T      current-node part of project_context (tsp: columns E:2E,
-                                        cvrp: columns 0:E)
+                                        the other envs: columns 0:E)
 
 so that the step query is a table-row read plus a per-episode constant (the reference
 re-does a 2E->E / (E+1)->E Linear per step, nn/env_embeddings/context.py:61-74,116-134).
@@ -28,7 +25,6 @@ The concatenated weight and its tf32 hi / lo split are cached per weight version
 
 from __future__ import annotations
 
-import os
 from dataclasses import dataclass
 
 import torch
@@ -79,10 +75,10 @@ class FusedPrecomputedCache:
 
     node_embeddings: torch.Tensor       # [B, N, E]
     graph_context: torch.Tensor | float  # [B, E] or 0
-    rollout_cache: torch.Tensor         # [B, N, W] (W = 4E; 5E for tsp with the first-node table)
+    rollout_cache: torch.Tensor         # [B, N, W] (W = 5E for tsp, 4E otherwise)
     q_placeholder: torch.Tensor | None  # [E] tsp
     w_capacity: torch.Tensor | None     # [E] cvrp
-    w_first: torch.Tensor | None = None  # [E, E] tsp: project_context.weight[:, :E] (first-node GEMV operand)
+    w_first: None = None                 # always None (see _precompute_cache)
     dyn_w: torch.Tensor | None = None    # [3E] sdvrp: dynamic-embedding weights [wk | wv | W_out^T wl]
     _logit_weight: torch.Tensor | None = None
     _logit_key: torch.Tensor | None = None
@@ -145,16 +141,14 @@ class FusedAttentionModelDecoder(nn.Module):
         self.cache_gemm = cache_gemm
 
     # ------------------------------------------------------------------ cache
-    def fused_weight(self, first_table: bool = True) -> torch.Tensor:
+    def fused_weight(self) -> torch.Tensor:
         """Wcat [W, E]: row blocks as listed in the module docstring."""
         wk, wv, wl = self.project_node_embeddings.weight.chunk(3, dim=0)
         wlf = self.pointer.project_out.weight.t() @ wl  # (L W_out) = h (W_out^T W_L)^T
         wc = self.context_embedding.project_context.weight
         blocks = [wk, wv, wlf]
         if self.env_name == "tsp":
-            if first_table:
-                blocks.append(wc[:, :E])
-            blocks.append(wc[:, E:2 * E])
+            blocks += [wc[:, :E], wc[:, E:2 * E]]
         else:
             blocks.append(wc[:, :E])
         return torch.cat(blocks, dim=0)
@@ -164,52 +158,50 @@ class FusedAttentionModelDecoder(nn.Module):
               self.context_embedding.project_context.weight)
         return tuple((p._version, p.data_ptr()) for p in ps)
 
-    def _fused_weight_cached(self, first_table: bool):
+    def _fused_weight_cached(self):
         """(Wcat, hi, lo) for the no-grad path, recomputed only when a parameter changed (optimizer step,
         load_state_dict, .to()): three small kernels per call otherwise sit inside every timed step."""
-        cache = self.__dict__.setdefault("_wcat_cache", {})
         ver = self._weight_version()
-        hit = cache.get(first_table)
+        hit = self.__dict__.get("_wcat_cache")
         if hit is None or hit[0] != ver:
             with torch.no_grad():
-                wcat = self.fused_weight(first_table).contiguous()
+                wcat = self.fused_weight().contiguous()
                 hi, lo = native.split_tf32(wcat) if wcat.is_cuda else (None, None)
             hit = (ver, wcat, hi, lo)
-            cache[first_table] = hit
+            self.__dict__["_wcat_cache"] = hit
         return hit[1], hit[2], hit[3]
 
     def _precompute_cache(self, embeddings: torch.Tensor, num_starts: int = 0,
                           first_table: bool | None = None) -> FusedPrecomputedCache:
-        """am/decoder.py:201-228.  `first_table` (tsp): include the first-node context table (required by the
-        multistart kernel); default True, CO_TSP_FIRST_TABLE=0 selects the narrow layout for single-start calls."""
-        if first_table is None:
-            first_table = num_starts > 1 or os.environ.get("CO_TSP_FIRST_TABLE", "1") != "0"
-        first_table = bool(first_table) and self.env_name == "tsp"
+        """am/decoder.py:201-228."""
+        # `first_table` and the always-None `FusedPrecomputedCache.w_first` are kept only for existing callers: the
+        # tsp cache always holds the first-node table, so `first_table=False` cannot be honoured
+        if first_table is not None and not first_table:
+            raise ValueError("first_table=False is not supported: the tsp rollout cache always holds the first-node table")
         needs_grad = torch.is_grad_enabled() and (embeddings.requires_grad or any(
             p.requires_grad for p in (self.project_node_embeddings.weight, self.pointer.project_out.weight,
                                       self.context_embedding.project_context.weight)))
         if self.cache_gemm == "tf32x3" and embeddings.is_cuda and not needs_grad:
             B, N, _ = embeddings.shape
-            _, w_hi, w_lo = self._fused_weight_cached(first_table)
+            _, w_hi, w_lo = self._fused_weight_cached()
             cache = native.gemm_tf32x3(embeddings.detach().reshape(B * N, E), w_hi, w_lo).view(B, N, -1)
         elif not needs_grad:
-            cache = torch.nn.functional.linear(embeddings, self._fused_weight_cached(first_table)[0])
+            cache = torch.nn.functional.linear(embeddings, self._fused_weight_cached()[0])
         else:
-            cache = torch.nn.functional.linear(embeddings, self.fused_weight(first_table))
+            cache = torch.nn.functional.linear(embeddings, self.fused_weight())
         if self.use_graph_context:
             graph_context = self.project_fixed_context(embeddings.mean(1))
         else:
             graph_context = 0
         wc = self.context_embedding.project_context.weight
-        q_ph = w_cap = w_first = None
+        q_ph = w_cap = None
         if self.env_name == "tsp":
             q_ph = (wc @ self.context_embedding.W_placeholder).contiguous()
-            w_first = wc[:, :E].contiguous()
         else:
             w_cap = wc[:, E].contiguous()
         return FusedPrecomputedCache(
             node_embeddings=embeddings, graph_context=graph_context, rollout_cache=cache, q_placeholder=q_ph,
-            w_capacity=w_cap, w_first=w_first, dyn_w=self._dynamic_weights() if self.is_dynamic_embedding else None,
+            w_capacity=w_cap, dyn_w=self._dynamic_weights() if self.is_dynamic_embedding else None,
             _logit_weight=self.project_node_embeddings.weight[2 * E:],
         )
 
@@ -233,7 +225,6 @@ class FusedAttentionModelDecoder(nn.Module):
             wp = self.context_embedding.W_placeholder.detach().contiguous()
             keep.append(wp)
             w.w_placeholder = wp.data_ptr()
-        w.project_out_t = None  # logit key is folded
         if self.is_dynamic_embedding:
             # [wk | wv | W_out^T wl]: the logit third folded like the logit key itself (module docstring, block 2)
             wdyn = self._dynamic_weights()

@@ -107,7 +107,7 @@ def eas_search(policy, env, td, *, use_eas_embedding: bool = True, use_eas_layer
     try:
         with torch.no_grad():
             hidden, _ = policy.encoder(td)
-            cached = dec._precompute_cache(hidden, first_table=True)
+            cached = dec._precompute_cache(hidden)
             cache = cached.rollout_cache.contiguous().clone()
             w_out = dec.pointer.project_out.weight.detach().clone()
             w_l = dec.project_node_embeddings.weight.detach()[2 * E:3 * E]

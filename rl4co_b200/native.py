@@ -52,8 +52,8 @@ class NativeLibraryError(RuntimeError):
 
 
 class DecoderWeights(Structure):
-    _fields_ = [("project_context_t", c_void_p), ("w_placeholder", c_void_p), ("project_out_t", c_void_p),
-                ("dynamic_w", c_void_p), ("dynamic_feature", c_void_p)]
+    _fields_ = [("project_context_t", c_void_p), ("w_placeholder", c_void_p), ("dynamic_w", c_void_p),
+                ("dynamic_feature", c_void_p)]
 
 
 class RolloutArgs(Structure):
@@ -66,7 +66,7 @@ class RolloutArgs(Structure):
         ("forced_actions", c_void_p), ("noise", c_void_p), ("seed", c_uint64), ("offset", c_uint64),
         ("actions_out", c_void_p), ("logp_out", c_void_p), ("reward_out", c_void_p), ("loglik_out", c_void_p),
         ("steps_out", c_void_p), ("max_steps_out", c_void_p), ("used_capacity_out", c_void_p),
-        ("node_emb", c_void_p), ("w_first", c_void_p), ("cache_width", c_int32), ("reserved0", c_int32),
+        ("cache_width", c_int32), ("reserved0", c_int32),
         ("dyn_w", c_void_p), ("node_limit", c_void_p),
     ]
 
@@ -742,8 +742,8 @@ def rollout(env_name, select_mode, cache, graph_ctx, q_placeholder, w_capacity, 
             tanh_clipping=10.0, temperature=1.0, seed=0, offset=0, node_emb=None, w_first=None, dyn_w=None,
             node_limit=None):
     """Launch the persistent rollout kernel; returns dict of device tensors (no host sync).
-    `cache` is [B_inst, N, W]: W = 4E ([K | V | L' | cur-table]; tsp then needs `node_emb` [B_inst, N, E] and
-    `w_first` [E, E] for the per-episode first-node GEMV) or, tsp only, 5E (with the first-node table)."""
+    `cache` is [B_inst, N, W]: tsp W = 5E ([K | V | L' | first-table | cur-table]), the other envs 4E
+    ([K | V | L' | cur-table]).  `node_emb` and `w_first` are ignored; they are accepted for existing callers."""
     dev = cache.device
     S = max(1, int(num_starts))
     B_traj = B_inst * S
@@ -774,16 +774,9 @@ def rollout(env_name, select_mode, cache, graph_ctx, q_placeholder, w_capacity, 
     a.reward_out, a.loglik_out = _ptr(reward, F32, "reward"), _ptr(loglik, F32, "loglik")
     a.steps_out, a.max_steps_out = _ptr(steps, I32, "steps"), _ptr(max_steps, I32, "max_steps")
     a.used_capacity_out = _ptr(used_out, F32, "used_out")
-    W = cache.shape[-1]
-    ok_w = (4 * EMBED_DIM, 5 * EMBED_DIM) if env_name == "tsp" else (4 * EMBED_DIM,)
-    if cache.dim() != 3 or tuple(cache.shape[:2]) != (B_inst, N) or W not in ok_w:
-        raise ValueError(f"cache shape {tuple(cache.shape)} != ({B_inst}, {N}, {' | '.join(map(str, ok_w))})")
-    if env_name == "tsp" and W == 4 * EMBED_DIM:
-        if node_emb is None or w_first is None:
-            raise ValueError("tsp cache of width 4E needs node_emb and w_first")
-        if tuple(node_emb.shape) != (B_inst, N, EMBED_DIM) or tuple(w_first.shape) != (EMBED_DIM, EMBED_DIM):
-            raise ValueError("node_emb must be [B_inst, N, E] and w_first [E, E]")
-        a.node_emb, a.w_first = _ptr(node_emb, F32, "node_emb"), _ptr(w_first, F32, "w_first")
+    W = (5 if env_name == "tsp" else 4) * EMBED_DIM
+    if tuple(cache.shape) != (B_inst, N, W):
+        raise ValueError(f"cache shape {tuple(cache.shape)} != ({B_inst}, {N}, {W})")
     a.cache_width = W
     if env_name == "sdvrp":
         if dyn_w is None or tuple(dyn_w.shape) != (3 * EMBED_DIM,):

@@ -134,8 +134,7 @@ class FusedAttentionModelPolicy(nn.Module):
         # decode-step bound: tsp N; cvrp 2(N-1) (every customer + a depot return each); sdvrp 3(N-1)+2 (a customer can
         # be split once per refill on top of that)
         T_max = {"tsp": N, "cvrp": 2 * (N - 1), "op": N + 1, "pctsp": N + 1}.get(env_name, 3 * (N - 1) + 2)  # op / pctsp: customers once + depot
-        # S > 1 runs the query-batched kernel, which reads the tsp first-node table (one row per start)
-        cached = self.decoder._precompute_cache(hidden, first_table=True if S > 1 else None)
+        cached = self.decoder._precompute_cache(hidden)
 
         forced = None
         if decode_type == "evaluate":
@@ -179,9 +178,7 @@ class FusedAttentionModelPolicy(nn.Module):
                 cached.q_placeholder, cached.w_capacity, td["locs"].contiguous(), demand, vcap, B, N, num_starts=S,
                 forced_start=forced_start, num_loc=num_loc, T_max=T_max, forced_actions=forced,
                 noise=noise.contiguous() if noise is not None else None, tanh_clipping=tanh_clipping,
-                temperature=temperature, seed=seed or 0, offset=philox_offset or 0,
-                node_emb=hidden.detach().contiguous() if env_name == "tsp" else None,
-                w_first=cached.w_first.detach() if cached.w_first is not None else None, dyn_w=cached.dyn_w,
+                temperature=temperature, seed=seed or 0, offset=philox_offset or 0, dyn_w=cached.dyn_w,
                 node_limit=node_limit)
         if env_name == "tsp":
             T = N

@@ -40,7 +40,7 @@ def _cache(pol, td):
     dec = pol.decoder
     with torch.no_grad():
         hidden, _ = pol.encoder(td)
-        cached = dec._precompute_cache(hidden, first_table=True)
+        cached = dec._precompute_cache(hidden)
         cache = cached.rollout_cache.contiguous().clone()
         L = torch.matmul(hidden, dec.project_node_embeddings.weight[2 * E:3 * E].t()).contiguous()
         cache[..., 2 * E:3 * E] = torch.matmul(L, dec.pointer.project_out.weight)

@@ -719,23 +719,3 @@ def test_check_solution_rejects_capacity_overflow(golden, dev):
     assert load > 1.0 + 1e-5, "merged route does not overflow in this fixture row"
     with pytest.raises(AssertionError):
         env.check_solution_validity(td, bad)
-
-
-@pytest.mark.parametrize("name", ["am_tsp20", "am_tsp50", "am_tsp100"])
-def test_rollout_narrow_cache_first_node_gemv(golden, dev, name, monkeypatch):
-    """CO_TSP_FIRST_TABLE=0: the 4E cache layout, where the kernel computes the first-node half of the context
-    projection as one 128x128 GEMV per episode (context.py:129-133) instead of reading a table row."""
-    g = golden(name)
-    pol = make_policy("tsp", g.weights(), dev)
-    wide, _, _ = fused_rollout(pol, "tsp", g, dev, "greedy")
-    monkeypatch.setenv("CO_TSP_FIRST_TABLE", "0")
-    with torch.inference_mode():
-        assert pol.decoder._precompute_cache(g["h"].to(dev)).rollout_cache.shape[-1] == 4 * 128
-    out, _, _ = fused_rollout(pol, "tsp", g, dev, "evaluate", actions=g["eval_actions"].to(dev))
-    torch.testing.assert_close(out["log_likelihood"].cpu(), g["eval_logprobs"], rtol=RTOL, atol=ATOL_LP)
-    torch.testing.assert_close(out["reward"].cpu(), g["eval_reward"], rtol=RTOL, atol=1e-6)
-    narrow, _, _ = fused_rollout(pol, "tsp", g, dev, "greedy")
-    _check_against_prefix_oracle(g.weights(), "tsp", g.inst(), g["h"], narrow, "greedy")
-    same = _rows_equal(narrow["actions"].cpu(), wide["actions"].cpu())
-    assert same.float().mean() >= 0.75
-    torch.testing.assert_close(narrow["log_likelihood"][same.to(dev)], wide["log_likelihood"][same.to(dev)], rtol=RTOL, atol=ATOL_LP)

@@ -218,9 +218,8 @@ def _slice_call(a, k, b0, b1, S):
             a[i] = a[i][b0:b1].contiguous()
     a[9] = b1 - b0
     k = dict(k)
-    for key in ("node_emb", "node_limit"):
-        if k.get(key) is not None:
-            k[key] = k[key][b0:b1].contiguous()
+    if k.get("node_limit") is not None:
+        k["node_limit"] = k["node_limit"][b0:b1].contiguous()
     if k.get("forced_actions") is not None:
         k["forced_actions"] = k["forced_actions"][rows].contiguous()
     if k.get("noise") is not None:
@@ -237,8 +236,8 @@ def test_persistent_loop_batch_composition(env_name, S, monkeypatch):
     """B_inst = 2 * 8 * SMs + 7 makes every CTA of the persistent grid handle at least two instances (it re-initialises
     shared memory, the cvrp demand-rank sort and the sdvrp dynamic terms per instance, and prefetches the next one).
     The same instances in chunks of at most SM-count instances (one per CTA) must give bit-identical actions, per-step
-    log-probs, rewards and log-likelihoods; so must the large run without the L2 prefetch. The last 64 instances, which
-    run in a late loop iteration, are checked against the oracle."""
+    log-probs, rewards and log-likelihoods. The last 64 instances, which run in a late loop iteration, are checked
+    against the oracle."""
     from rl4co_b200 import native
 
     sms = native.lib().co_device_sm_count()
@@ -268,11 +267,6 @@ def test_persistent_loop_batch_composition(env_name, S, monkeypatch):
                 chunked[key][rows] = res[key]
         for key in OUT_KEYS:
             assert torch.equal(big[key], chunked[key]), f"{mode}: {key} depends on the batch composition"
-        monkeypatch.setenv("CO_ROLLOUT_PREFETCH", "0")
-        nopf = native.rollout(*a, **k)
-        monkeypatch.delenv("CO_ROLLOUT_PREFETCH")
-        for key in OUT_KEYS:
-            assert torch.equal(big[key], nopf[key]), f"{mode}: {key} changes without the prefetch"
         tail_out = {"actions": big["actions"][tail_rows].cpu(), "log_likelihood": big["logprobs"][tail_rows].cpu(),
                     "reward": big["reward"][tail_rows].cpu()}
         forced = mode == "greedy" and S > 1

@@ -55,6 +55,20 @@ def test_bad_arguments_return_error_codes_without_a_gpu(libpath):
     assert L.co_tsp_step(None, None, None, None, None, None, None, 4, 10, None) == -1
 
 
+@pytest.mark.parametrize("num_starts", [1, 8])
+def test_rollout_rejects_a_tsp_cache_without_the_first_node_table(libpath, num_starts):
+    """tsp reads the 5E cache only; the arguments are checked before any CUDA call, so fake pointers suffice."""
+    from rl4co_b200 import native
+
+    a = native.RolloutArgs()
+    a.env_kind, a.select_mode, a.B_inst, a.num_starts, a.N, a.T_max = native.ENV_TSP, native.SELECT_GREEDY, 2, num_starts, 20, 20
+    a.tanh_clipping, a.temperature, a.cache_width = 10.0, 1.0, 4 * 128
+    for name in ("cache", "q_placeholder", "locs", "actions_out", "logp_out", "reward_out", "loglik_out"):
+        setattr(a, name, 4096)
+    assert native.lib().co_rollout(ctypes.byref(a), None) == -1
+    assert b"5E" in native.lib().co_last_error_string()
+
+
 def test_tensordict_batch_semantics():
     from rl4co_b200.tensordict import TensorDict
 
@@ -170,8 +184,9 @@ def test_encoder_matches_reference_golden_cpu(golden, name, norm):
     torch.testing.assert_close(h, g["h"], rtol=1e-5, atol=1e-5)
 
 
-def test_fused_weight_blocks_cpu(golden):
-    """the single cache GEMM reproduces K / V and the folded logit key / context tables."""
+def test_fused_weight_blocks_single_layout_cpu(golden):
+    """the single cache GEMM reproduces K / V and the folded logit key / context tables of the one tsp layout (5E);
+    `first_table=False` is rejected."""
     from rl4co_b200.decoder import FusedAttentionModelDecoder
 
     g = golden("am_tsp20")
@@ -180,10 +195,12 @@ def test_fused_weight_blocks_cpu(golden):
     dec.load_state_dict(w)
     h = g["h"]
     with torch.inference_mode():
-        c = dec._precompute_cache(h)  # default layout: with the first-node table
-        c4 = dec._precompute_cache(h, first_table=False)  # narrow layout (per-episode GEMV in the kernel)
+        c = dec._precompute_cache(h)
+        assert torch.equal(dec._precompute_cache(h, first_table=True).rollout_cache, c.rollout_cache)
+        with pytest.raises(ValueError, match="first_table"):
+            dec._precompute_cache(h, first_table=False)
     E = 128
-    assert c.rollout_cache.shape[-1] == 5 * E and c4.rollout_cache.shape[-1] == 4 * E
+    assert c.rollout_cache.shape[-1] == 5 * E and c.w_first is None
     kvl = torch.nn.functional.linear(h, w["project_node_embeddings.weight"])
     torch.testing.assert_close(c.glimpse_key, kvl[..., :E], rtol=1e-5, atol=1e-5)
     torch.testing.assert_close(c.glimpse_val, kvl[..., E:2 * E], rtol=1e-5, atol=1e-5)
@@ -192,15 +209,12 @@ def test_fused_weight_blocks_cpu(golden):
     wc = w["context_embedding.project_context.weight"]
     torch.testing.assert_close(c.rollout_cache[..., 3 * E:4 * E], h @ wc[:, :E].t(), rtol=1e-4, atol=1e-4)
     torch.testing.assert_close(c.rollout_cache[..., 4 * E:5 * E], h @ wc[:, E:].t(), rtol=1e-4, atol=1e-4)
-    torch.testing.assert_close(c4.rollout_cache[..., :3 * E], c.rollout_cache[..., :3 * E])
-    torch.testing.assert_close(c4.rollout_cache[..., 3 * E:], c.rollout_cache[..., 4 * E:])
-    assert torch.equal(c4.w_first, wc[:, :E])
     # the concatenated weight is cached per weight version and refreshed when a parameter changes
-    w0 = dec._fused_weight_cached(False)[0]
-    assert dec._fused_weight_cached(False)[0] is w0
+    w0 = dec._fused_weight_cached()[0]
+    assert dec._fused_weight_cached()[0] is w0
     with torch.no_grad():
         dec.pointer.project_out.weight.mul_(2.0)
-    assert dec._fused_weight_cached(False)[0] is not w0
+    assert dec._fused_weight_cached()[0] is not w0
     torch.testing.assert_close(c.q_placeholder, wc @ w["context_embedding.W_placeholder"], rtol=1e-5, atol=1e-5)
 
 

@@ -58,7 +58,7 @@ def run(env_name, N, B, A, iters, split_iters, chunks):
     tda = StateAugmentation(num_augment=A, augment_fn="dihedral8")(td)
     with torch.no_grad():
         hidden, _ = pol.encoder(tda)
-        cached = dec._precompute_cache(hidden, first_table=True)
+        cached = dec._precompute_cache(hidden)
         cache = cached.rollout_cache.contiguous().clone()
         w_out = dec.pointer.project_out.weight.detach().clone()
         L = torch.nn.Parameter(torch.matmul(hidden, dec.project_node_embeddings.weight[2 * E:3 * E].t()).contiguous())
