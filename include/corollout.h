@@ -291,7 +291,15 @@ typedef struct co_rollout_args {
    * [B_inst, N-1], `vehicle_capacity` the budget at the depot max_length[:, 0], reward_out the collected prize;
    * pctsp: penalty per node [B_inst, N] (depot 0); `demand` = real prizes [B_inst, N-1], `vehicle_capacity` = prize_required */
   const float* node_limit;
+  /* EAS-Lay (rl4co/models/zoo/eas/nn.py, decoder.py:12-31): per-instance residual layer on the concatenated head output
+   * o (E channels, (h g) order) of every decode step of every trajectory of instance b, before project_out:
+   *   o' = o + relu(o W1 + b1) W2 + b2,  u_n = o' . Lf[n] / sqrt(E)
+   * packed [B_inst, CO_EAS_LAYER_FLOATS] fp32 as [W1 (E x E, (in, out)) | b1 (E) | W2 (E x E, (in, out)) | b2 (E)],
+   * 16-byte aligned.  NULL: no layer.  Non-NULL only for tsp / cvrp with num_starts > 1 (else CO_ERR_UNSUPPORTED);
+   * misaligned: CO_ERR_BAD_ARG. */
+  const float* eas_layer;
 } co_rollout_args;
+#define CO_EAS_LAYER_FLOATS (2 * CO_EMBED_DIM * CO_EMBED_DIM + 2 * CO_EMBED_DIM)
 
 /* Efficient active search, embedding variant (EAS-Emb; rl4co/models/zoo/eas/search.py:198-235): gradient of a
  * weighted sum of trajectory log-likelihoods with respect to the folded logit key Lf = L W_out (block 2 of the cache).
@@ -336,6 +344,38 @@ typedef struct co_eas_grad_args {
   int32_t* bad_rows;         /* [1] out (accumulated) or NULL                            */
 } co_eas_grad_args;
 int co_eas_key_grad(const co_eas_grad_args* args, void* stream);
+
+/* Efficient active search, layer variant (EAS-Lay; rl4co/models/zoo/eas/nn.py, search.py:198-235): gradient of
+ * sum_j coef[j] loglik[j] with respect to the per-instance layer of co_rollout_args.eas_layer.  Rows, coef, the
+ * replay, the rules for infeasible rows (loglik NaN, *bad_rows + 1, no contribution) and the errors are those of
+ * co_eas_key_grad, with u_n computed from o' = o + relu(o W1 + b1) W2 + b2 (a = o W1 + b1, z = relu(a)).  Per
+ * replayed step, with g_n as in co_eas_key_grad:
+ *   do' = sum_n g_n Lf[n];  dW2 += z^T do', db2 += do';  dz = (do' W2^T) * [a > 0];  dW1 += o^T dz, db1 += dz
+ * layer / dlayer [B_inst, CO_EAS_LAYER_FLOATS] packed as co_rollout_args.eas_layer, 16-byte aligned.  One CTA owns one
+ * instance and sums every entry in the fixed order (row, step): bit-identical across launches and independent of the
+ * other instances of the batch.  No host synchronisation. */
+typedef struct co_eas_layer_grad_args {
+  int32_t env_kind;          /* CO_ENV_TSP | CO_ENV_CVRP                                  */
+  int32_t B_inst;
+  int32_t num_rows;
+  int32_t N;
+  int32_t T;
+  int32_t cache_width;
+  float tanh_clipping;
+  float temperature;
+  const float* cache;        /* [B_inst, N, cache_width]                                 */
+  const float* graph_ctx;    /* [B_inst, E] or NULL                                      */
+  const float* w_capacity;   /* [E] cvrp                                                 */
+  const float* demand;       /* [B_inst, N-1] cvrp                                       */
+  const float* vehicle_capacity; /* [B_inst] cvrp or NULL (= 1.0)                        */
+  const int64_t* actions;    /* [R * B_inst, T]                                          */
+  const float* coef;         /* [R * B_inst]                                             */
+  const float* layer;        /* [B_inst, CO_EAS_LAYER_FLOATS]                            */
+  float* dlayer;             /* [B_inst, CO_EAS_LAYER_FLOATS] out                        */
+  float* loglik;             /* [R * B_inst] out                                         */
+  int32_t* bad_rows;         /* [1] out (accumulated) or NULL                            */
+} co_eas_layer_grad_args;
+int co_eas_layer_grad(const co_eas_layer_grad_args* args, void* stream);
 
 int co_cache_width(int env_kind); /* floats per node row of the rollout cache (tsp 5E, the other envs 4E) */
 /* largest N the persistent kernel is instantiated for (else CO_ERR_UNSUPPORTED) */

@@ -36,6 +36,11 @@ extern "C" int co_rollout(const co_rollout_args* args, void* stream) {
   if (A.select_mode == CO_SELECT_SAMPLE_NOISE && !A.noise) return fail(CO_ERR_BAD_ARG, "co_rollout: noise required%s");
   if (A.select_mode == CO_SELECT_SAMPLE_PHILOX) A.noise = nullptr;
   if ((A.flags & CO_ROLLOUT_FORCED_START) && A.num_loc < 1) return fail(CO_ERR_BAD_ARG, "co_rollout: num_loc required for forced starts%s");
+  if (A.eas_layer) {  // EAS-Lay lives in the query-batched kernel only
+    if ((A.env_kind != CO_ENV_TSP && A.env_kind != CO_ENV_CVRP) || A.num_starts < 2)
+      return fail(CO_ERR_UNSUPPORTED, "co_rollout: eas_layer needs tsp / cvrp with num_starts > 1%s");
+    if ((uintptr_t)A.eas_layer & 15) return fail(CO_ERR_BAD_ARG, "co_rollout: eas_layer must be 16-byte aligned%s");
+  }
   if (A.B_inst == 0) return CO_OK;
   cudaStream_t st = (cudaStream_t)stream;
   // S > 1 trajectories per instance: tsp and cvrp run the query-batched kernel, which advances 4 of them per pass, so

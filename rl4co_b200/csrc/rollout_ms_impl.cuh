@@ -19,6 +19,12 @@
 //   * trajectories that are done (CVRP: variable length) are still computed but their results are
 //     discarded by predication; the group ends when all of its trajectories are done.
 // Layout of results is unchanged: row j = s * B + b (start-major, rl4co/utils/ops.py:10-29).
+//
+// LAYER (EAS-Lay, co_rollout_args.eas_layer): the head outputs are normalised in the glimpse (the layer is not linear,
+// so the 1 / sum(exp) factor cannot stay on the logit shares), written to LayerMS::o, and each pass runs
+// o' = o + relu(o W1 + b1) W2 + b2 for its Q trajectories with the whole block (thread (channel c, trajectory pair)),
+// W1 / W2 of the instance read through L1 / L2 (128 KiB: they do not fit beside SmemMS<4>); o' takes the place of
+// the head outputs in the logit shares.  Three block barriers more per pass.  LAYER = false is the kernel as before.
 #pragma once
 #include "rollout_impl.cuh"
 
@@ -53,7 +59,31 @@ struct SmemMS {
   float ll_acc[MSQ];
 };
 
-template <int SPL, int ENV, int MODE>
+// EAS-Lay buffers, behind SmemMS<SPL> in the LAYER variant
+struct LayerMS {
+  alignas(16) float o[MSQ][E];  // normalised head outputs of the pass, (h g) order
+  alignas(16) float z[MSQ][E];  // relu(o W1 + b1)
+};
+template <int SPL>
+__host__ __device__ constexpr size_t layer_ms_offset() { return (sizeof(SmemMS<SPL>) + 15) & ~size_t(15); }
+
+// y0 / y1 = x0 / x1 . W[:, c] for a row-major (in, out) [E, E] W in global memory; four partial sums (i mod 4)
+__device__ __forceinline__ void layer_matvec2(const float* x0, const float* x1, const float* __restrict__ W, int c,
+                                              float& y0, float& y1) {
+  float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 2
+  for (int i = 0; i < E; i += 4) {
+    const float4 u = *reinterpret_cast<const float4*>(x0 + i), v = *reinterpret_cast<const float4*>(x1 + i);
+    const float w0 = __ldg(W + (i + 0) * E + c), w1 = __ldg(W + (i + 1) * E + c);
+    const float w2 = __ldg(W + (i + 2) * E + c), w3 = __ldg(W + (i + 3) * E + c);
+    s0[0] = fmaf(u.x, w0, s0[0]); s0[1] = fmaf(u.y, w1, s0[1]); s0[2] = fmaf(u.z, w2, s0[2]); s0[3] = fmaf(u.w, w3, s0[3]);
+    s1[0] = fmaf(v.x, w0, s1[0]); s1[1] = fmaf(v.y, w1, s1[1]); s1[2] = fmaf(v.z, w2, s1[2]); s1[3] = fmaf(v.w, w3, s1[3]);
+  }
+  y0 = (s0[0] + s0[1]) + (s0[2] + s0[3]);
+  y1 = (s1[0] + s1[1]) + (s1[2] + s1[3]);
+}
+
+template <int SPL, int ENV, int MODE, bool LAYER = false>
 __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_args A) {
   using C = CfgMS<SPL>;
   constexpr int NS = C::NS, TPG = C::TPG, GA = C::GA;
@@ -63,6 +93,7 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
   constexpr int Q = MSQ;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SmemMS<SPL>& sm = *reinterpret_cast<SmemMS<SPL>*>(smem_raw);
+  [[maybe_unused]] LayerMS& lay = *reinterpret_cast<LayerMS*>(smem_raw + layer_ms_offset<SPL>());  // LAYER only
 
   const int tid = threadIdx.x, lane = tid & 31, h = tid >> 5;
   const int N = A.N, B_inst = A.B_inst, S = A.num_starts, T_max = A.T_max;
@@ -330,13 +361,40 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
             r2[u] = (s0 + s1) + (s2 + s3);
           }
           const float x0 = __shfl_xor_sync(FULL, r2[0], 16), x1 = __shfl_xor_sync(FULL, r2[1], 16);
-          if (lane < 16) {  // un-normalised head outputs (d == lane here)
-            sm.oh[h][jp][d] = r2[0] + x0;
-            sm.oh[h][jp + 1][d] = r2[1] + x1;
+          if constexpr (LAYER) {
+            rinv[jp] = __fdividef(1.0f, esum[0]);
+            rinv[jp + 1] = __fdividef(1.0f, esum[1]);
+            if (lane < 16) {  // normalised head outputs, channel h * D + d
+              lay.o[jp][h * D + d] = (r2[0] + x0) * rinv[jp];
+              lay.o[jp + 1][h * D + d] = (r2[1] + x1) * rinv[jp + 1];
+            }
+          } else {
+            if (lane < 16) {  // un-normalised head outputs (d == lane here)
+              sm.oh[h][jp][d] = r2[0] + x0;
+              sm.oh[h][jp + 1][d] = r2[1] + x1;
+            }
+            rinv[jp] = __fdividef(1.0f, esum[0]);
+            rinv[jp + 1] = __fdividef(1.0f, esum[1]);
           }
-          rinv[jp] = __fdividef(1.0f, esum[0]);
-          rinv[jp + 1] = __fdividef(1.0f, esum[1]);
           __syncwarp();  // the two tiles are reused by the next pair; oh is complete after the last pair
+        }
+        if constexpr (LAYER) {
+          // ---------------- EAS-Lay: o' = o + relu(o W1 + b1) W2 + b2; thread (channel c, trajectories j0, j0 + 1)
+          const float* Lw = A.eas_layer + (size_t)b * CO_EAS_LAYER_FLOATS;
+          const int c = tid & (E - 1), j0 = 2 * (tid >> 7);
+          __syncthreads();  // every head output of the pass is in lay.o
+          float y0, y1;
+          layer_matvec2(lay.o[j0], lay.o[j0 + 1], Lw, c, y0, y1);
+          const float b1 = __ldg(Lw + E * E + c);
+          y0 += b1; y1 += b1;
+          lay.z[j0][c] = y0 > 0.f ? y0 : 0.f;
+          lay.z[j0 + 1][c] = y1 > 0.f ? y1 : 0.f;
+          __syncthreads();  // z complete
+          layer_matvec2(lay.z[j0], lay.z[j0 + 1], Lw + E * E + E, c, y0, y1);
+          const float b2 = __ldg(Lw + 2 * E * E + E + c);
+          sm.oh[c >> 4][j0][c & (D - 1)] = lay.o[j0][c] + (y0 + b2);
+          sm.oh[c >> 4][j0 + 1][c & (D - 1)] = lay.o[j0 + 1][c] + (y1 + b2);
+          __syncthreads();  // o' of every trajectory is in oh
         }
         // ---------------- head h's share of every pointer logit, for the Q trajectories: the head's slice of the folded
         // logit key is read once per pass (conflict-free LDS.128, lane l = node l + 32 k), the head outputs as broadcasts
@@ -364,7 +422,10 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
 #pragma unroll
           for (int j = 0; j < Q; ++j)
 #pragma unroll
-            for (int k = 0; k < SPL; ++k) sm.part[j][h][lane + 32 * k] = (pl2[j][k].x + pl2[j][k].y) * rinv[j];
+            for (int k = 0; k < SPL; ++k) {
+              if constexpr (LAYER) sm.part[j][h][lane + 32 * k] = pl2[j][k].x + pl2[j][k].y;  // o' is normalised
+              else sm.part[j][h][lane + 32 * k] = (pl2[j][k].x + pl2[j][k].y) * rinv[j];
+            }
         }
         __syncthreads();  // B1: every head's share of every logit of all trajectories is in shared memory
 
@@ -491,10 +552,10 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
   }
 }
 
-template <int SPL, int ENV, int MODE>
+template <int SPL, int ENV, int MODE, bool LAYER>
 static int launch_ms(const co_rollout_args& A, cudaStream_t st) {
-  auto kern = rollout_ms_kernel<SPL, ENV, MODE>;
-  const size_t smem = sizeof(SmemMS<SPL>);
+  auto kern = rollout_ms_kernel<SPL, ENV, MODE, LAYER>;
+  const size_t smem = LAYER ? layer_ms_offset<SPL>() + sizeof(LayerMS) : sizeof(SmemMS<SPL>);
   static PerDeviceOnce once;
   bool& configured = once.flag();
   if (!configured) {
@@ -513,7 +574,9 @@ static int dispatch_ms(const co_rollout_args& A, cudaStream_t st) {
   const int spl = A.N <= 32 ? 1 : (A.N <= 64 ? 2 : 4);
   const int mode = A.select_mode == CO_SELECT_GREEDY ? CO_MODE_GREEDY
                    : (A.select_mode == CO_SELECT_EVALUATE ? CO_MODE_EVALUATE : CO_MODE_SAMPLE);
-#define CO_CASE(S_, M_) if (spl == S_ && mode == M_) return launch_ms<S_, ENV, M_>(A, st)
+  const bool layer = A.eas_layer != nullptr;
+#define CO_CASE(S_, M_) \
+  if (spl == S_ && mode == M_) return layer ? launch_ms<S_, ENV, M_, true>(A, st) : launch_ms<S_, ENV, M_, false>(A, st)
   CO_CASE(1, CO_MODE_GREEDY); CO_CASE(2, CO_MODE_GREEDY); CO_CASE(4, CO_MODE_GREEDY);
   CO_CASE(1, CO_MODE_SAMPLE); CO_CASE(2, CO_MODE_SAMPLE); CO_CASE(4, CO_MODE_SAMPLE);
   CO_CASE(1, CO_MODE_EVALUATE); CO_CASE(2, CO_MODE_EVALUATE); CO_CASE(4, CO_MODE_EVALUATE);

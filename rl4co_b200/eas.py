@@ -1,21 +1,32 @@
-"""Efficient active search with embedding updates (EAS-Emb; Hottung et al., ICLR 2022; rl4co/models/zoo/eas/search.py).
+"""Efficient active search (EAS; Hottung et al., ICLR 2022; rl4co/models/zoo/eas/search.py): EAS-Emb and EAS-Lay.
 
-`eas_search(policy, env, td, **hparams)` fine-tunes, per instance, the pointer logit key L = node_emb W_L^T of a frozen
-policy: each iteration samples POMO multistart tours from the current key with the whole-episode rollout kernel
-(`co_rollout`, in-kernel Philox), then takes one optimizer step on L.  The loss is rl4co's
+`eas_search(policy, env, td, **hparams)` fine-tunes per-instance parameters of a frozen policy: each iteration samples
+POMO multistart tours with the whole-episode rollout kernel (`co_rollout`, in-kernel Philox), then takes one optimizer
+step on those parameters.
+  * EAS-Emb (`use_eas_embedding=True`, the default): the pointer logit key L = node_emb W_L^T.
+  * EAS-Lay (`use_eas_layer=True, use_eas_embedding=False`): a residual layer per augmented instance on the
+    concatenated head output o of every decode step, o' = o + relu(o W1 + b1) W2 + b2 before project_out
+    (rl4co/models/zoo/eas/nn.py, decoder.py:12-31), initialised as rl4co's `EASLayerNet` (`eas_layer_init`): W1, b1
+    xavier-uniform over the [B * A, E, E] / [B * A, 1, E] tensors, W2 = b2 = 0, so iteration 0 decodes as the policy.
+    The rollout kernel applies the layer in its query-batched (multistart) variant; its gradient comes from
+    `co_eas_layer_grad`, which replays the rows teacher-forced through the layer.
+The loss is rl4co's
 
     loss = -mean((r - baseline) * ll_sampled) + eas_lambda * -mean(ll_incumbent)
 
-whose gradient with respect to the folded key Lf = L W_out comes from one CUDA kernel (`co_eas_key_grad`) that replays
-the sampled tours and the incumbent teacher-forced and keeps the N x E accumulator on chip; no [B, S*T, N] logits or
-glimpses are ever stored.  dL = dLf W_out^T.
+whose gradient comes from one CUDA kernel that replays the sampled tours and the incumbent teacher-forced; no
+[B, S*T, N] logits or glimpses are ever stored.  EAS-Emb: `co_eas_key_grad` gives the gradient with respect to the
+folded key Lf = L W_out, keeping the N x E accumulator on chip, and dL = dLf W_out^T.  EAS-Lay: `co_eas_layer_grad`
+gives the gradient of the packed [W1 | b1 | W2 | b2] of every instance.
 
 Deviations from rl4co's `EAS`:
   * a function over one batch, not a Lightning `TransductiveModel` (Lightning is not a dependency);
   * iteration 0 has no incumbent row: rl4co imitates an extra sampled start-0 tour there (and its `% num_starts` makes
     one CVRP start the depot);
   * the samples come from the in-kernel Philox stream keyed by (seed, iteration), not `torch.multinomial`;
-  * only EAS-Emb on the logit key, `num_parallel_runs=1`, tsp / cvrp and N <= 128 are supported.
+  * EAS-Emb on the logit key or EAS-Lay, not both at once; `num_parallel_runs=1`, tsp / cvrp and N <= 128;
+  * EAS-Lay keeps the four layer tensors in one packed parameter [B * A, 2 E^2 + 2 E]; an element-wise optimizer
+    (Adam, the default, SGD, ...) steps it exactly as it would step the four tensors.
 """
 
 from __future__ import annotations
@@ -52,6 +63,28 @@ def eas_coefficients(reward: torch.Tensor, baseline: str, eas_lambda: float, wit
     return coef
 
 
+def eas_layer_init(num_instances: int, device=None) -> torch.Tensor:
+    """rl4co's `EASLayerNet(num_instances, E)` initialisation, drawn the same way from torch's CPU generator (randn of
+    W1 and b1, then xavier_uniform_ over the whole [n, E, E] / [n, 1, E] tensors, so the bound depends on n; W2 = b2 =
+    0), packed per instance as [W1 (E x E, (in, out)) | b1 | W2 | b2] -> [n, native.EAS_LAYER_FLOATS] on `device`."""
+    w1 = torch.randn(num_instances, E, E)
+    b1 = torch.randn(num_instances, 1, E)
+    torch.nn.init.xavier_uniform_(w1)
+    torch.nn.init.xavier_uniform_(b1)
+    packed = torch.zeros(num_instances, native.EAS_LAYER_FLOATS, device=device)
+    packed[:, :E * E] = w1.reshape(num_instances, E * E).to(device)
+    packed[:, E * E:E * E + E] = b1.reshape(num_instances, E).to(device)
+    return packed
+
+
+def unpack_eas_layer(packed: torch.Tensor) -> dict:
+    """[n, native.EAS_LAYER_FLOATS] -> {"W1": [n, E, E], "b1": [n, 1, E], "W2": [n, E, E], "b2": [n, 1, E]} (views),
+    the shapes of rl4co's `EASLayerNet` parameters."""
+    n = packed.shape[0]
+    return {"W1": packed[:, :E * E].view(n, E, E), "b1": packed[:, E * E:E * E + E].view(n, 1, E),
+            "W2": packed[:, E * E + E:2 * E * E + E].view(n, E, E), "b2": packed[:, 2 * E * E + E:].view(n, 1, E)}
+
+
 def _make_optimizer(optimizer, params, kwargs):
     if isinstance(optimizer, str):
         return getattr(torch.optim, optimizer)(params, **kwargs)
@@ -62,18 +95,21 @@ def eas_search(policy, env, td, *, use_eas_embedding: bool = True, use_eas_layer
                eas_emb_cache_keys=("logit_key",), eas_lambda: float = 0.013, max_iters: int = 200,
                augment_size: int = 8, augment_dihedral: bool = True, num_parallel_runs: int = 1,
                baseline: str = "multistart", max_runtime: float = 86_400, optimizer="Adam",
-               optimizer_kwargs=None, seed: int | None = None, return_logit_key: bool = False) -> dict:
-    """EAS-Emb over the reset batch `td` [B] (see the module docstring).
+               optimizer_kwargs=None, seed: int | None = None, return_logit_key: bool = False,
+               return_layer: bool = False) -> dict:
+    """EAS-Emb or EAS-Lay over the reset batch `td` [B] (see the module docstring).
 
     Returns {"max_reward": [B], "best_solutions": [B, T] (0-padded; T = N for tsp, 2 (N - 1) for cvrp),
     "reward_history": [iterations run, B] (the best reward found so far after each iteration)}, plus "logit_key"
-    ([A * B, N, E], aug-major) with `return_logit_key=True`.  The policy's parameters are not modified.  The loop
-    synchronises with the host once per iteration (the `max_runtime` check)."""
-    if use_eas_layer:
-        raise NotImplementedError("EAS-Lay needs a per-instance layer inside the rollout kernel; use EAS-Emb")
-    if not use_eas_embedding:
+    ([A * B, N, E], aug-major) with `return_logit_key=True` (EAS-Emb) and "layer" (`unpack_eas_layer` of the trained
+    [A * B, ...] layer, aug-major) with `return_layer=True` (EAS-Lay).  The policy's parameters are not modified.  The
+    loop synchronises with the host once per iteration (the `max_runtime` check)."""
+    if use_eas_layer and use_eas_embedding:
+        raise NotImplementedError("EAS-Emb and EAS-Lay together are not supported (the key gradient would have to go "
+                                  "through the layer); pass use_eas_embedding=False for EAS-Lay")
+    if not use_eas_embedding and not use_eas_layer:
         raise ValueError("At least one of `use_eas_embedding` or `use_eas_layer` must be True.")
-    if list(eas_emb_cache_keys) != ["logit_key"]:
+    if use_eas_embedding and list(eas_emb_cache_keys) != ["logit_key"]:
         raise NotImplementedError(f"EAS-Emb fine-tunes the logit key only, got cache keys {list(eas_emb_cache_keys)}")
     if num_parallel_runs != 1:
         raise NotImplementedError("num_parallel_runs != 1 is not supported (rl4co's incumbent bookkeeping assumes one run)")
@@ -99,6 +135,7 @@ def eas_search(policy, env, td, *, use_eas_embedding: bool = True, use_eas_layer
     BA = A * B
     T = N if env_name == "tsp" else 2 * (N - 1)
     dev = td["locs"].device
+    layer = torch.nn.Parameter(eas_layer_init(BA, dev)) if use_eas_layer else None  # before any other draw
     if seed is None:
         seed = int(torch.randint(0, 2**62, (1,)).item())
     dec = policy.decoder
@@ -111,14 +148,14 @@ def eas_search(policy, env, td, *, use_eas_embedding: bool = True, use_eas_layer
             cache = cached.rollout_cache.contiguous().clone()
             w_out = dec.pointer.project_out.weight.detach().clone()
             w_l = dec.project_node_embeddings.weight.detach()[2 * E:3 * E]
-            L = torch.nn.Parameter(torch.matmul(hidden.detach(), w_l.t()).contiguous())
+            L = torch.nn.Parameter(torch.matmul(hidden.detach(), w_l.t()).contiguous()) if use_eas_embedding else None
             graph_ctx = cached.graph_context_or_none
             graph_ctx = graph_ctx.detach().contiguous() if graph_ctx is not None else None
             q_ph = cached.q_placeholder.detach() if cached.q_placeholder is not None else None
             w_cap = cached.w_capacity.detach() if cached.w_capacity is not None else None
     finally:
         policy.train(was_training)
-    opt = _make_optimizer(optimizer, [L], optimizer_kwargs)
+    opt = _make_optimizer(optimizer, [L if use_eas_embedding else layer], optimizer_kwargs)
     locs = td["locs"].contiguous()
     demand = td["demand"].contiguous() if env_name == "cvrp" else None
     vcap = td["vehicle_capacity"].reshape(-1).contiguous() if env_name == "cvrp" else None
@@ -131,21 +168,24 @@ def eas_search(policy, env, td, *, use_eas_embedding: bool = True, use_eas_layer
     t_start = time.time()
     for it in range(max_iters):
         with torch.no_grad():
-            cache[..., 2 * E:3 * E] = torch.matmul(L.detach(), w_out)  # folded key Lf = L W_out (cache block 2)
+            if use_eas_embedding:
+                cache[..., 2 * E:3 * E] = torch.matmul(L.detach(), w_out)  # folded key Lf = L W_out (cache block 2)
             res = native.rollout(env_name, native.SELECT_SAMPLE_PHILOX, cache, graph_ctx, q_ph, w_cap, locs, demand,
                                  vcap, BA, N, num_starts=S, forced_start=True, num_loc=num_loc, T_max=T,
                                  tanh_clipping=policy.tanh_clipping, temperature=policy.temperature, seed=seed,
-                                 offset=it)
+                                 offset=it, layer=layer.detach() if use_eas_layer else None)
             reward = res["reward"].view(S, A, B)
             rows = res["actions"]
             coef = eas_coefficients(reward, baseline, eas_lambda, with_incumbent=it > 0)
             if it > 0:
                 rows = torch.cat([rows, best.repeat(A, 1)])  # the incumbent replayed in every augmentation
-            dLf, _ = native.eas_key_grad(env_name, cache, rows, coef.contiguous(), graph_ctx=graph_ctx,
-                                         w_capacity=w_cap, demand=demand, vehicle_capacity=vcap,
-                                         tanh_clipping=policy.tanh_clipping, temperature=policy.temperature,
-                                         bad_rows=bad)
-            L.grad = torch.matmul(dLf, w_out.t())
+            kw = dict(graph_ctx=graph_ctx, w_capacity=w_cap, demand=demand, vehicle_capacity=vcap,
+                      tanh_clipping=policy.tanh_clipping, temperature=policy.temperature, bad_rows=bad)
+            if use_eas_embedding:
+                dLf, _ = native.eas_key_grad(env_name, cache, rows, coef.contiguous(), **kw)
+                L.grad = torch.matmul(dLf, w_out.t())
+            else:
+                layer.grad, _ = native.eas_layer_grad(env_name, cache, rows, coef.contiguous(), layer.detach(), **kw)
         opt.step()
         with torch.no_grad():
             # incumbent: the best tour of instance b over starts, augmentations and iterations (strict improvement)
@@ -157,10 +197,12 @@ def eas_search(policy, env, td, *, use_eas_embedding: bool = True, use_eas_layer
             best = torch.where(improve[:, None], cand, best)
             history.append(max_reward.clone())
         if int(bad.item()):  # the one host synchronisation of the iteration
-            raise RuntimeError("co_eas_key_grad replayed an infeasible trajectory")
+            raise RuntimeError("the EAS gradient kernel replayed an infeasible trajectory")
         if time.time() - t_start > max_runtime:
             break
     out = {"max_reward": max_reward, "best_solutions": best, "reward_history": torch.stack(history) if history else torch.empty(0, B, device=dev)}
-    if return_logit_key:
+    if return_logit_key and use_eas_embedding:
         out["logit_key"] = L.detach()
+    if return_layer and use_eas_layer:
+        out["layer"] = unpack_eas_layer(layer.detach())
     return out

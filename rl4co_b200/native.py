@@ -43,7 +43,7 @@ EXPORTS = [
     "co_ffn_fused", "co_ffn_tile_weights", "co_ffn_tiled_weight_floats", "co_generate_uniform", "co_generate_demand", "co_dihedral8",
     "co_sdvrp_step", "co_sdvrp_action_mask", "co_attn_fwd", "co_attn_bwd", "co_instance_norm", "co_op_step", "co_op_action_mask", "co_op_reward", "co_pctsp_step", "co_pctsp_action_mask",
     "co_tsp_two_opt", "co_generate_locs", "co_symmetric_augment", "co_cvrp_local_search",
-    "co_eas_key_grad",
+    "co_eas_key_grad", "co_eas_layer_grad",
 ]
 
 
@@ -67,7 +67,7 @@ class RolloutArgs(Structure):
         ("actions_out", c_void_p), ("logp_out", c_void_p), ("reward_out", c_void_p), ("loglik_out", c_void_p),
         ("steps_out", c_void_p), ("max_steps_out", c_void_p), ("used_capacity_out", c_void_p),
         ("cache_width", c_int32), ("reserved0", c_int32),
-        ("dyn_w", c_void_p), ("node_limit", c_void_p),
+        ("dyn_w", c_void_p), ("node_limit", c_void_p), ("eas_layer", c_void_p),
     ]
 
 
@@ -76,6 +76,17 @@ class EasGradArgs(Structure):
                 ("cache_width", c_int32), ("tanh_clipping", c_float), ("temperature", c_float)] + [
         (n, c_void_p) for n in ("cache", "graph_ctx", "w_capacity", "demand", "vehicle_capacity", "actions", "coef",
                                 "dLf", "loglik", "bad_rows")]
+
+
+class EasLayerGradArgs(Structure):
+    _fields_ = [("env_kind", c_int32), ("B_inst", c_int32), ("num_rows", c_int32), ("N", c_int32), ("T", c_int32),
+                ("cache_width", c_int32), ("tanh_clipping", c_float), ("temperature", c_float)] + [
+        (n, c_void_p) for n in ("cache", "graph_ctx", "w_capacity", "demand", "vehicle_capacity", "actions", "coef",
+                                "layer", "dlayer", "loglik", "bad_rows")]
+
+
+#: floats of one instance's packed EAS-Lay layer [W1 (E x E) | b1 (E) | W2 (E x E) | b2 (E)] (CO_EAS_LAYER_FLOATS)
+EAS_LAYER_FLOATS = 2 * EMBED_DIM * EMBED_DIM + 2 * EMBED_DIM
 
 
 class AttnArgs(Structure):
@@ -176,6 +187,7 @@ def lib() -> ctypes.CDLL:
     L.co_op_reward.argtypes = [c_void_p] * 3 + [c_int, c_int, c_int, c_void_p]
     L.co_instance_norm.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_long, c_int, c_float, c_void_p]
     L.co_eas_key_grad.argtypes = [POINTER(EasGradArgs), c_void_p]
+    L.co_eas_layer_grad.argtypes = [POINTER(EasLayerGradArgs), c_void_p]
     L.co_attn_fwd.argtypes = [POINTER(AttnArgs), c_void_p]
     L.co_attn_bwd.argtypes = [POINTER(AttnArgs), c_void_p]
     L.co_cache_width.argtypes = [c_int]
@@ -458,8 +470,30 @@ def eas_key_grad(env_name, cache, actions, coef, graph_ctx=None, w_capacity=None
     with dLf = d(sum_j coef[j] loglik[j]) / d(folded logit key, block 2 of `cache`).  `cache` [B_inst, N, W] (tsp: 5E
     layout, cvrp: 4E); actions [R*B_inst, T] int64 start-major with column 0 a forced start; coef [R*B_inst] float32.
     An infeasible row gets loglik NaN and adds 1 to `bad_rows` (optional int32 [1] device counter); no host sync."""
+    B_inst, N, W, R, T = _check_eas_inputs(env_name, cache, actions, coef, graph_ctx, w_capacity, demand,
+                                           vehicle_capacity, bad_rows, "co_eas_key_grad")
+    dLf = torch.empty(B_inst, N, EMBED_DIM, dtype=F32, device=cache.device)
+    loglik = torch.empty(R * B_inst, dtype=F32, device=cache.device)
+    a = EasGradArgs()
+    a.env_kind, a.B_inst, a.num_rows, a.N, a.T, a.cache_width = ENV_KIND[env_name], B_inst, R, N, T, W
+    a.tanh_clipping, a.temperature = float(tanh_clipping), float(temperature)
+    a.cache = _ptr(cache, F32, "cache")
+    a.graph_ctx = _ptr(graph_ctx, F32, "graph_ctx")
+    a.w_capacity = _ptr(w_capacity, F32, "w_capacity") if env_name == "cvrp" else None
+    a.demand = _ptr(demand, F32, "demand") if env_name == "cvrp" else None
+    a.vehicle_capacity = _ptr(vehicle_capacity, F32, "vehicle_capacity") if env_name == "cvrp" else None
+    a.actions = _ptr(actions, I64, "actions")
+    a.coef = _ptr(coef, F32, "coef")
+    a.dLf, a.loglik = _ptr(dLf, F32, "dLf"), _ptr(loglik, F32, "loglik")
+    a.bad_rows = _ptr(bad_rows, I32, "bad_rows")
+    _check(lib().co_eas_key_grad(ctypes.byref(a), _stream()), "co_eas_key_grad")
+    return dLf, loglik
+
+
+def _check_eas_inputs(env_name, cache, actions, coef, graph_ctx, w_capacity, demand, vehicle_capacity, bad_rows, what):
+    """Shape checks shared by eas_key_grad / eas_layer_grad -> (B_inst, N, W, R, T)."""
     if env_name not in ("tsp", "cvrp"):
-        raise NotImplementedError(f"co_eas_key_grad covers tsp and cvrp, not {env_name!r}")
+        raise NotImplementedError(f"{what} covers tsp and cvrp, not {env_name!r}")
     if cache.dim() != 3:
         raise ValueError(f"cache: expected [B_inst, N, W], got {tuple(cache.shape)}")
     B_inst, N, W = cache.shape
@@ -479,9 +513,28 @@ def eas_key_grad(env_name, cache, actions, coef, graph_ctx=None, w_capacity=None
             raise ValueError(f"vehicle_capacity: expected [{B_inst}], got {tuple(vehicle_capacity.shape)}")
     if bad_rows is not None and tuple(bad_rows.shape) != (1,):
         raise ValueError("bad_rows: expected an int32 [1] counter")
-    dLf = torch.empty(B_inst, N, EMBED_DIM, dtype=F32, device=cache.device)
+    return B_inst, N, W, R, T
+
+
+def _check_layer(layer, B_inst, name="layer"):
+    if layer is None or tuple(layer.shape) != (B_inst, EAS_LAYER_FLOATS):
+        got = None if layer is None else tuple(layer.shape)
+        raise ValueError(f"{name}: expected the packed EAS-Lay layer [{B_inst}, {EAS_LAYER_FLOATS}], got {got}")
+
+
+@_on_device_of_first_tensor
+def eas_layer_grad(env_name, cache, actions, coef, layer, graph_ctx=None, w_capacity=None, demand=None,
+                   vehicle_capacity=None, tanh_clipping=10.0, temperature=1.0, bad_rows=None):
+    """co_eas_layer_grad: teacher-forced replay of R trajectories per instance through the per-instance EAS-Lay layer
+    -> (dlayer [B_inst, EAS_LAYER_FLOATS], loglik [R*B_inst]) with dlayer = d(sum_j coef[j] loglik[j]) / d(layer).
+    `layer` [B_inst, EAS_LAYER_FLOATS] float32 packs [W1 | b1 | W2 | b2] per instance (W as (in, out)); the other
+    arguments are those of `eas_key_grad`.  An infeasible row gets loglik NaN and adds 1 to `bad_rows`; no host sync."""
+    B_inst, N, W, R, T = _check_eas_inputs(env_name, cache, actions, coef, graph_ctx, w_capacity, demand,
+                                           vehicle_capacity, bad_rows, "co_eas_layer_grad")
+    _check_layer(layer, B_inst)
+    dlayer = torch.empty(B_inst, EAS_LAYER_FLOATS, dtype=F32, device=cache.device)
     loglik = torch.empty(R * B_inst, dtype=F32, device=cache.device)
-    a = EasGradArgs()
+    a = EasLayerGradArgs()
     a.env_kind, a.B_inst, a.num_rows, a.N, a.T, a.cache_width = ENV_KIND[env_name], B_inst, R, N, T, W
     a.tanh_clipping, a.temperature = float(tanh_clipping), float(temperature)
     a.cache = _ptr(cache, F32, "cache")
@@ -491,10 +544,11 @@ def eas_key_grad(env_name, cache, actions, coef, graph_ctx=None, w_capacity=None
     a.vehicle_capacity = _ptr(vehicle_capacity, F32, "vehicle_capacity") if env_name == "cvrp" else None
     a.actions = _ptr(actions, I64, "actions")
     a.coef = _ptr(coef, F32, "coef")
-    a.dLf, a.loglik = _ptr(dLf, F32, "dLf"), _ptr(loglik, F32, "loglik")
+    a.layer, a.dlayer = _ptr(layer, F32, "layer"), _ptr(dlayer, F32, "dlayer")
+    a.loglik = _ptr(loglik, F32, "loglik")
     a.bad_rows = _ptr(bad_rows, I32, "bad_rows")
-    _check(lib().co_eas_key_grad(ctypes.byref(a), _stream()), "co_eas_key_grad")
-    return dLf, loglik
+    _check(lib().co_eas_layer_grad(ctypes.byref(a), _stream()), "co_eas_layer_grad")
+    return dlayer, loglik
 
 
 @_on_device_of_first_tensor
@@ -740,13 +794,19 @@ def reward_stats(reward, out2):
 def rollout(env_name, select_mode, cache, graph_ctx, q_placeholder, w_capacity, locs, demand, vehicle_capacity,
             B_inst, N, num_starts=1, forced_start=False, num_loc=0, T_max=None, forced_actions=None, noise=None,
             tanh_clipping=10.0, temperature=1.0, seed=0, offset=0, node_emb=None, w_first=None, dyn_w=None,
-            node_limit=None):
+            node_limit=None, layer=None):
     """Launch the persistent rollout kernel; returns dict of device tensors (no host sync).
     `cache` is [B_inst, N, W]: tsp W = 5E ([K | V | L' | first-table | cur-table]), the other envs 4E
-    ([K | V | L' | cur-table]).  `node_emb` and `w_first` are ignored; they are accepted for existing callers."""
+    ([K | V | L' | cur-table]).  `node_emb` and `w_first` are ignored; they are accepted for existing callers.
+    `layer` [B_inst, EAS_LAYER_FLOATS] (tsp / cvrp, num_starts > 1): the per-instance EAS-Lay layer applied to the
+    head output of every decode step (see `eas_layer_grad`)."""
     dev = cache.device
     S = max(1, int(num_starts))
     B_traj = B_inst * S
+    if layer is not None:
+        if env_name not in ("tsp", "cvrp") or S < 2:
+            raise NotImplementedError("the EAS-Lay layer runs in the multistart kernel: tsp / cvrp with num_starts > 1")
+        _check_layer(layer, B_inst)
     if T_max is None:
         T_max = {"tsp": N, "cvrp": 2 * (N - 1), "op": N + 1, "pctsp": N + 1}.get(env_name, 3 * (N - 1) + 2)
     actions = torch.empty(B_traj, T_max, dtype=I64, device=dev)
@@ -786,6 +846,7 @@ def rollout(env_name, select_mode, cache, graph_ctx, q_placeholder, w_capacity, 
         if node_limit is None or tuple(node_limit.shape) != (B_inst, N):
             raise ValueError(f"{env_name} needs node_limit [{B_inst}, {N}] (op: max_length, pctsp: penalty)")
         a.node_limit = _ptr(node_limit, F32, "node_limit")
+    a.eas_layer = _ptr(layer, F32, "layer")
     if forced_actions is not None and tuple(forced_actions.shape) != (B_traj, T_max):
         raise ValueError(f"forced_actions must be [{B_traj}, {T_max}], got {tuple(forced_actions.shape)}")
     if noise is not None and (noise.dim() != 3 or noise.shape[1] != B_traj or noise.shape[2] != N):
