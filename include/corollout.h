@@ -298,8 +298,22 @@ typedef struct co_rollout_args {
    * 16-byte aligned.  NULL: no layer.  Non-NULL only for tsp / cvrp with num_starts > 1 (else CO_ERR_UNSUPPORTED);
    * misaligned: CO_ERR_BAD_ARG. */
   const float* eas_layer;
+  /* PolyNet (Hottung et al. 2024; rl4co/models/nn/attention.py PolyNetAttention): the glimpse g = o W_out^T of every
+   * decode step of trajectory s goes through one residual MLP conditioned on strategy s % poly_k,
+   *   g' = g + (relu(g W1 + c[s % poly_k]) W2 + b2),  u_n = g' . L[n] / sqrt(E)
+   * with c[i] = b1 + poly_layer_1.weight[:, E:] . binary_vector[i] and L the UN-folded logit key (block 2 of the cache
+   * holds L itself, not L W_out).  Weights shared by every instance, packed fp32 and 16-byte aligned as
+   *   [W_out^T (E x E) | W1 (E x P) | W2 (P x E) | b2 (E) | c (poly_k x P)],  P = CO_POLY_DIM, matrices (in, out),
+   * CO_POLY_FIXED_FLOATS + poly_k * CO_POLY_DIM floats.  NULL: no poly layer (poly_k is then not read).  Non-NULL only
+   * for tsp / cvrp with num_starts > 1 and eas_layer NULL (else CO_ERR_UNSUPPORTED); misaligned or poly_k < 1:
+   * CO_ERR_BAD_ARG. */
+  const float* poly;
+  int32_t poly_k;
+  int32_t reserved1;
 } co_rollout_args;
 #define CO_EAS_LAYER_FLOATS (2 * CO_EMBED_DIM * CO_EMBED_DIM + 2 * CO_EMBED_DIM)
+#define CO_POLY_DIM 256
+#define CO_POLY_FIXED_FLOATS (CO_EMBED_DIM * CO_EMBED_DIM + 2 * CO_EMBED_DIM * CO_POLY_DIM + CO_EMBED_DIM)
 
 /* Efficient active search, embedding variant (EAS-Emb; rl4co/models/zoo/eas/search.py:198-235): gradient of a
  * weighted sum of trajectory log-likelihoods with respect to the folded logit key Lf = L W_out (block 2 of the cache).

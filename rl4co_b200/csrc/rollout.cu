@@ -41,6 +41,12 @@ extern "C" int co_rollout(const co_rollout_args* args, void* stream) {
       return fail(CO_ERR_UNSUPPORTED, "co_rollout: eas_layer needs tsp / cvrp with num_starts > 1%s");
     if ((uintptr_t)A.eas_layer & 15) return fail(CO_ERR_BAD_ARG, "co_rollout: eas_layer must be 16-byte aligned%s");
   }
+  if (A.poly) {  // PolyNet lives in the query-batched kernel only, and not together with EAS-Lay
+    if ((A.env_kind != CO_ENV_TSP && A.env_kind != CO_ENV_CVRP) || A.num_starts < 2 || A.eas_layer)
+      return fail(CO_ERR_UNSUPPORTED, "co_rollout: poly needs tsp / cvrp with num_starts > 1 and no eas_layer%s");
+    if ((uintptr_t)A.poly & 15) return fail(CO_ERR_BAD_ARG, "co_rollout: poly must be 16-byte aligned%s");
+    if (A.poly_k < 1) return fail(CO_ERR_BAD_ARG, "co_rollout: poly_k must be >= 1%s");
+  }
   if (A.B_inst == 0) return CO_OK;
   cudaStream_t st = (cudaStream_t)stream;
   // S > 1 trajectories per instance: tsp and cvrp run the query-batched kernel, which advances 4 of them per pass, so

@@ -25,6 +25,13 @@
 // o' = o + relu(o W1 + b1) W2 + b2 for its Q trajectories with the whole block (thread (channel c, trajectory pair)),
 // W1 / W2 of the instance read through L1 / L2 (128 KiB: they do not fit beside SmemMS<4>); o' takes the place of
 // the head outputs in the logit shares.  Three block barriers more per pass.  LAYER = false is the kernel as before.
+//
+// POLY (PolyNet, co_rollout_args.poly): the head outputs are normalised into PolyMS::o as for LAYER; each pass then
+// computes g = o W_out^T (thread (channel c, trajectory pair)), u = relu(g W1 + c[s % k]) over CO_POLY_DIM channels
+// (thread = channel, all Q trajectories) and g' = g + (u W2 + b2) (thread (channel c, trajectory pair)), and g' takes the
+// place of the head outputs in the logit shares against the un-folded logit key in block 2 of the cache.  The weights
+// (320 KiB + k KiB) are shared by all instances and read through L1 / L2 like EAS-Lay's; four block barriers more per
+// pass.
 #pragma once
 #include "rollout_impl.cuh"
 
@@ -64,6 +71,13 @@ struct LayerMS {
   alignas(16) float o[MSQ][E];  // normalised head outputs of the pass, (h g) order
   alignas(16) float z[MSQ][E];  // relu(o W1 + b1)
 };
+// PolyNet buffers, behind SmemMS<SPL> in the POLY variant; `o` sits where LayerMS::o does
+struct PolyMS {
+  alignas(16) float o[MSQ][E];            // normalised head outputs of the pass, (h g) order
+  alignas(16) float g[MSQ][E];            // glimpse o W_out^T
+  alignas(16) float u[MSQ][CO_POLY_DIM];  // relu(g W1 + c[s % k])
+};
+static_assert(offsetof(PolyMS, o) == offsetof(LayerMS, o), "the glimpse writes both through LayerMS::o");
 template <int SPL>
 __host__ __device__ constexpr size_t layer_ms_offset() { return (sizeof(SmemMS<SPL>) + 15) & ~size_t(15); }
 
@@ -83,7 +97,30 @@ __device__ __forceinline__ void layer_matvec2(const float* x0, const float* x1, 
   y1 = (s1[0] + s1[1]) + (s1[2] + s1[3]);
 }
 
-template <int SPL, int ENV, int MODE, bool LAYER = false>
+// y[j] = x[j * ldx + .] . W[:, c], j < NJ, for a row-major (in, out) [IN, OUT] W in global memory; four partial sums
+// (i mod 4) per row
+template <int IN, int OUT, int NJ>
+__device__ __forceinline__ void poly_matvec(const float* x, int ldx, const float* __restrict__ W, int c,
+                                            float (&y)[NJ]) {
+  float s[NJ][4];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+#pragma unroll 4
+  for (int i = 0; i < IN; i += 4) {
+    const float w0 = __ldg(W + (i + 0) * OUT + c), w1 = __ldg(W + (i + 1) * OUT + c);
+    const float w2 = __ldg(W + (i + 2) * OUT + c), w3 = __ldg(W + (i + 3) * OUT + c);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const float4 u = *reinterpret_cast<const float4*>(x + j * ldx + i);
+      s[j][0] = fmaf(u.x, w0, s[j][0]); s[j][1] = fmaf(u.y, w1, s[j][1]);
+      s[j][2] = fmaf(u.z, w2, s[j][2]); s[j][3] = fmaf(u.w, w3, s[j][3]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) y[j] = (s[j][0] + s[j][1]) + (s[j][2] + s[j][3]);
+}
+
+template <int SPL, int ENV, int MODE, bool LAYER = false, bool POLY = false>
 __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_args A) {
   using C = CfgMS<SPL>;
   constexpr int NS = C::NS, TPG = C::TPG, GA = C::GA;
@@ -94,6 +131,7 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SmemMS<SPL>& sm = *reinterpret_cast<SmemMS<SPL>*>(smem_raw);
   [[maybe_unused]] LayerMS& lay = *reinterpret_cast<LayerMS*>(smem_raw + layer_ms_offset<SPL>());  // LAYER only
+  [[maybe_unused]] PolyMS& pm = *reinterpret_cast<PolyMS*>(smem_raw + layer_ms_offset<SPL>());     // POLY only
 
   const int tid = threadIdx.x, lane = tid & 31, h = tid >> 5;
   const int N = A.N, B_inst = A.B_inst, S = A.num_starts, T_max = A.T_max;
@@ -361,7 +399,7 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
             r2[u] = (s0 + s1) + (s2 + s3);
           }
           const float x0 = __shfl_xor_sync(FULL, r2[0], 16), x1 = __shfl_xor_sync(FULL, r2[1], 16);
-          if constexpr (LAYER) {
+          if constexpr (LAYER || POLY) {
             rinv[jp] = __fdividef(1.0f, esum[0]);
             rinv[jp + 1] = __fdividef(1.0f, esum[1]);
             if (lane < 16) {  // normalised head outputs, channel h * D + d
@@ -396,6 +434,31 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
           sm.oh[c >> 4][j0 + 1][c & (D - 1)] = lay.o[j0 + 1][c] + (y1 + b2);
           __syncthreads();  // o' of every trajectory is in oh
         }
+        if constexpr (POLY) {
+          // ---------------- PolyNet: g = o W_out^T, u = relu(g W1 + c[s % k]), g' = g + (u W2 + b2)
+          constexpr int P = CO_POLY_DIM;
+          const float* Pw = A.poly;
+          const int c = tid & (E - 1), j0 = 2 * (tid >> 7);
+          __syncthreads();  // every head output of the pass is in pm.o
+          float y2[2];
+          poly_matvec<E, E, 2>(pm.o[j0], E, Pw, c, y2);
+          pm.g[j0][c] = y2[0];
+          pm.g[j0 + 1][c] = y2[1];
+          __syncthreads();  // g complete
+          float y4[Q];
+          poly_matvec<E, P, Q>(pm.g[0], E, Pw + E * E, tid, y4);
+#pragma unroll
+          for (int j = 0; j < Q; ++j) {
+            const float v = y4[j] + __ldg(Pw + CO_POLY_FIXED_FLOATS + (size_t)((g0 + j) % A.poly_k) * P + tid);
+            pm.u[j][tid] = v > 0.f ? v : 0.f;
+          }
+          __syncthreads();  // u complete
+          poly_matvec<P, E, 2>(pm.u[j0], P, Pw + E * E + E * P, c, y2);
+          const float b2 = __ldg(Pw + E * E + 2 * E * P + c);
+          sm.oh[c >> 4][j0][c & (D - 1)] = pm.g[j0][c] + (y2[0] + b2);
+          sm.oh[c >> 4][j0 + 1][c & (D - 1)] = pm.g[j0 + 1][c] + (y2[1] + b2);
+          __syncthreads();  // g' of every trajectory is in oh
+        }
         // ---------------- head h's share of every pointer logit, for the Q trajectories: the head's slice of the folded
         // logit key is read once per pass (conflict-free LDS.128, lane l = node l + 32 k), the head outputs as broadcasts
         {
@@ -423,7 +486,7 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
           for (int j = 0; j < Q; ++j)
 #pragma unroll
             for (int k = 0; k < SPL; ++k) {
-              if constexpr (LAYER) sm.part[j][h][lane + 32 * k] = pl2[j][k].x + pl2[j][k].y;  // o' is normalised
+              if constexpr (LAYER || POLY) sm.part[j][h][lane + 32 * k] = pl2[j][k].x + pl2[j][k].y;  // o' / g' are normalised
               else sm.part[j][h][lane + 32 * k] = (pl2[j][k].x + pl2[j][k].y) * rinv[j];
             }
         }
@@ -552,10 +615,11 @@ __global__ void __launch_bounds__(256, 1) rollout_ms_kernel(const co_rollout_arg
   }
 }
 
-template <int SPL, int ENV, int MODE, bool LAYER>
+template <int SPL, int ENV, int MODE, bool LAYER, bool POLY = false>
 static int launch_ms(const co_rollout_args& A, cudaStream_t st) {
-  auto kern = rollout_ms_kernel<SPL, ENV, MODE, LAYER>;
-  const size_t smem = LAYER ? layer_ms_offset<SPL>() + sizeof(LayerMS) : sizeof(SmemMS<SPL>);
+  auto kern = rollout_ms_kernel<SPL, ENV, MODE, LAYER, POLY>;
+  const size_t smem = LAYER ? layer_ms_offset<SPL>() + sizeof(LayerMS)
+                            : (POLY ? layer_ms_offset<SPL>() + sizeof(PolyMS) : sizeof(SmemMS<SPL>));
   static PerDeviceOnce once;
   bool& configured = once.flag();
   if (!configured) {
@@ -574,9 +638,11 @@ static int dispatch_ms(const co_rollout_args& A, cudaStream_t st) {
   const int spl = A.N <= 32 ? 1 : (A.N <= 64 ? 2 : 4);
   const int mode = A.select_mode == CO_SELECT_GREEDY ? CO_MODE_GREEDY
                    : (A.select_mode == CO_SELECT_EVALUATE ? CO_MODE_EVALUATE : CO_MODE_SAMPLE);
-  const bool layer = A.eas_layer != nullptr;
-#define CO_CASE(S_, M_) \
-  if (spl == S_ && mode == M_) return layer ? launch_ms<S_, ENV, M_, true>(A, st) : launch_ms<S_, ENV, M_, false>(A, st)
+  const bool layer = A.eas_layer != nullptr, poly = A.poly != nullptr;
+#define CO_CASE(S_, M_)                                                                      \
+  if (spl == S_ && mode == M_)                                                               \
+  return layer ? launch_ms<S_, ENV, M_, true>(A, st)                                         \
+               : (poly ? launch_ms<S_, ENV, M_, false, true>(A, st) : launch_ms<S_, ENV, M_, false>(A, st))
   CO_CASE(1, CO_MODE_GREEDY); CO_CASE(2, CO_MODE_GREEDY); CO_CASE(4, CO_MODE_GREEDY);
   CO_CASE(1, CO_MODE_SAMPLE); CO_CASE(2, CO_MODE_SAMPLE); CO_CASE(4, CO_MODE_SAMPLE);
   CO_CASE(1, CO_MODE_EVALUATE); CO_CASE(2, CO_MODE_EVALUATE); CO_CASE(4, CO_MODE_EVALUATE);

@@ -68,6 +68,7 @@ class RolloutArgs(Structure):
         ("steps_out", c_void_p), ("max_steps_out", c_void_p), ("used_capacity_out", c_void_p),
         ("cache_width", c_int32), ("reserved0", c_int32),
         ("dyn_w", c_void_p), ("node_limit", c_void_p), ("eas_layer", c_void_p),
+        ("poly", c_void_p), ("poly_k", c_int32), ("reserved1", c_int32),
     ]
 
 
@@ -87,6 +88,10 @@ class EasLayerGradArgs(Structure):
 
 #: floats of one instance's packed EAS-Lay layer [W1 (E x E) | b1 (E) | W2 (E x E) | b2 (E)] (CO_EAS_LAYER_FLOATS)
 EAS_LAYER_FLOATS = 2 * EMBED_DIM * EMBED_DIM + 2 * EMBED_DIM
+#: hidden width of the PolyNet layer (CO_POLY_DIM) and the floats of its packed weights without the per-strategy biases,
+#: [W_out^T (E x E) | W1 (E x P) | W2 (P x E) | b2 (E)] (CO_POLY_FIXED_FLOATS); k strategies add k * POLY_DIM floats
+POLY_DIM = 256
+POLY_FIXED_FLOATS = EMBED_DIM * EMBED_DIM + 2 * EMBED_DIM * POLY_DIM + EMBED_DIM
 
 
 class AttnArgs(Structure):
@@ -516,6 +521,15 @@ def _check_eas_inputs(env_name, cache, actions, coef, graph_ctx, w_capacity, dem
     return B_inst, N, W, R, T
 
 
+def _check_poly(poly, poly_k):
+    k = int(poly_k) if poly_k is not None else 0
+    if k < 1:
+        raise ValueError(f"poly_k: expected the number of PolyNet strategies (>= 1), got {poly_k!r}")
+    if poly.dim() != 1 or poly.numel() != POLY_FIXED_FLOATS + k * POLY_DIM:
+        raise ValueError(f"poly: expected the packed PolyNet weights [{POLY_FIXED_FLOATS + k * POLY_DIM}] for k = {k}, "
+                         f"got {tuple(poly.shape)}")
+
+
 def _check_layer(layer, B_inst, name="layer"):
     if layer is None or tuple(layer.shape) != (B_inst, EAS_LAYER_FLOATS):
         got = None if layer is None else tuple(layer.shape)
@@ -794,12 +808,15 @@ def reward_stats(reward, out2):
 def rollout(env_name, select_mode, cache, graph_ctx, q_placeholder, w_capacity, locs, demand, vehicle_capacity,
             B_inst, N, num_starts=1, forced_start=False, num_loc=0, T_max=None, forced_actions=None, noise=None,
             tanh_clipping=10.0, temperature=1.0, seed=0, offset=0, node_emb=None, w_first=None, dyn_w=None,
-            node_limit=None, layer=None):
+            node_limit=None, layer=None, poly=None, poly_k=None):
     """Launch the persistent rollout kernel; returns dict of device tensors (no host sync).
     `cache` is [B_inst, N, W]: tsp W = 5E ([K | V | L' | first-table | cur-table]), the other envs 4E
     ([K | V | L' | cur-table]).  `node_emb` and `w_first` are ignored; they are accepted for existing callers.
     `layer` [B_inst, EAS_LAYER_FLOATS] (tsp / cvrp, num_starts > 1): the per-instance EAS-Lay layer applied to the
-    head output of every decode step (see `eas_layer_grad`)."""
+    head output of every decode step (see `eas_layer_grad`).
+    `poly` [POLY_FIXED_FLOATS + poly_k * POLY_DIM] (tsp / cvrp, num_starts > 1, not with `layer`): the PolyNet layer
+    packed as `co_rollout_args.poly` (see `rl4co_b200.polynet.pack_poly`), applied to the glimpse of every decode step
+    of trajectory s with strategy s % poly_k; `cache` block 2 must then hold the un-folded logit key."""
     dev = cache.device
     S = max(1, int(num_starts))
     B_traj = B_inst * S
@@ -807,6 +824,11 @@ def rollout(env_name, select_mode, cache, graph_ctx, q_placeholder, w_capacity, 
         if env_name not in ("tsp", "cvrp") or S < 2:
             raise NotImplementedError("the EAS-Lay layer runs in the multistart kernel: tsp / cvrp with num_starts > 1")
         _check_layer(layer, B_inst)
+    if poly is not None:
+        if env_name not in ("tsp", "cvrp") or S < 2 or layer is not None:
+            raise NotImplementedError("the PolyNet layer runs in the multistart kernel: tsp / cvrp with num_starts > 1, "
+                                      "without an EAS-Lay layer")
+        _check_poly(poly, poly_k)
     if T_max is None:
         T_max = {"tsp": N, "cvrp": 2 * (N - 1), "op": N + 1, "pctsp": N + 1}.get(env_name, 3 * (N - 1) + 2)
     actions = torch.empty(B_traj, T_max, dtype=I64, device=dev)
@@ -847,6 +869,8 @@ def rollout(env_name, select_mode, cache, graph_ctx, q_placeholder, w_capacity, 
             raise ValueError(f"{env_name} needs node_limit [{B_inst}, {N}] (op: max_length, pctsp: penalty)")
         a.node_limit = _ptr(node_limit, F32, "node_limit")
     a.eas_layer = _ptr(layer, F32, "layer")
+    a.poly = _ptr(poly, F32, "poly")
+    a.poly_k = int(poly_k) if poly is not None else 0
     if forced_actions is not None and tuple(forced_actions.shape) != (B_traj, T_max):
         raise ValueError(f"forced_actions must be [{B_traj}, {T_max}], got {tuple(forced_actions.shape)}")
     if noise is not None and (noise.dim() != 3 or noise.shape[1] != B_traj or noise.shape[2] != N):

@@ -172,6 +172,7 @@ class FusedAttentionModelPolicy(nn.Module):
             vcap = td["prize_required"].reshape(-1).contiguous()
             node_limit = td["penalty"].contiguous()
         num_loc = getattr(env.generator, "num_loc", N - (1 if vrp or env_name in ("op", "pctsp") else 0))
+        extra = self.decoder.rollout_extras(S) if hasattr(self.decoder, "rollout_extras") else {}
         with torch.no_grad():
             res = native.rollout(
                 env_name, mode, cached.rollout_cache.detach().contiguous(), cached.graph_context_or_none,
@@ -179,7 +180,7 @@ class FusedAttentionModelPolicy(nn.Module):
                 forced_start=forced_start, num_loc=num_loc, T_max=T_max, forced_actions=forced,
                 noise=noise.contiguous() if noise is not None else None, tanh_clipping=tanh_clipping,
                 temperature=temperature, seed=seed or 0, offset=philox_offset or 0, dyn_w=cached.dyn_w,
-                node_limit=node_limit)
+                node_limit=node_limit, **extra)
         if env_name == "tsp":
             T = N
         elif decode_type == "evaluate":

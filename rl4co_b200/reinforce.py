@@ -144,10 +144,14 @@ REPLAY_KEYS = ("locs", "demand", "vehicle_capacity", "max_length", "real_prize",
 
 def evaluate_log_likelihood(policy, td: TensorDict, env, actions: torch.Tensor, hidden=None,
                             return_sum: bool = True, temperature=None, tanh_clipping=None,
-                            forced_first=None) -> torch.Tensor:
+                            forced_first=None, strategy=None) -> torch.Tensor:
     """log pi(actions | instance) with autograd, equal (<= fp32 round-off) to what the rollout
     kernel reported for the same actions.  `td` is the reset state (multistart: the [B] state,
-    actions [S*B, T] in the reference's start-major order)."""
+    actions [S*B, T] in the reference's start-major order).
+
+    A PolyNet decoder (`rl4co_b200.polynet`) applies its poly layer to the glimpse of row j = s * B + b with strategy
+    s % k, as its rollout does; `strategy` [S*B] (int64, start-major like the rows) replays row j with strategy[j]
+    instead, so that any row of a rollout can be replayed on its own."""
     env_name = env.name
     if env_name not in ("tsp", "cvrp", "sdvrp", "op", "pctsp"):
         raise NotImplementedError(f"the vectorised teacher-forced pass replays tsp / cvrp / sdvrp / op / pctsp state only "
@@ -222,6 +226,16 @@ def evaluate_log_likelihood(policy, td: TensorDict, env, actions: torch.Tensor, 
         o = F.scaled_dot_product_attention(heads(q), heads(K), heads(V), attn_mask=mask[:, None])
         o = o.transpose(1, 2).reshape(B, Q, E)
     glimpse = dec.pointer.project_out(o)
+    if hasattr(dec.pointer, "poly"):  # PolyNet: queries are instance-major [B, S * T], one strategy per row s
+        if strategy is None:
+            strat = (torch.arange(S, device=glimpse.device) % dec.pointer.k).repeat_interleave(T)[None]  # [1, Q]
+        else:
+            if tuple(strategy.shape) != (S * B,):
+                raise ValueError(f"strategy: expected [{S * B}] (one per row), got {tuple(strategy.shape)}")
+            strat = strategy.to(glimpse.device).view(S, B).t().repeat_interleave(T, dim=1)          # [B, Q]
+        glimpse = dec.pointer.poly(glimpse, strat)
+    elif strategy is not None:
+        raise ValueError("strategy is only defined for a PolyNet decoder")
     logits = torch.bmm(glimpse, L.transpose(1, 2))
     if remaining is not None:
         logits = logits + (glimpse * wl).sum(-1, keepdim=True) * remaining

@@ -58,6 +58,15 @@ AT.self_attention_packed(qkv).sum().backward()
 native.instance_norm(torch.randn(9, 100, 128, device=dev), torch.ones(128, device=dev), torch.zeros(128, device=dev))
 torch.cuda.synchronize()
 print("attention / norm ok")
+# PolyNet: the multistart kernel's poly variant (co_rollout_args.poly), k = 3 strategies wrapping over 7 starts
+from rl4co_b200.polynet import FusedPolyNetPolicy
+
+for env_name in ("tsp", "cvrp"):
+    env = get_env(env_name, generator_params=dict(num_loc=50), check_solution=True)
+    pol = FusedPolyNetPolicy(k=3, env_name=env_name, num_encoder_layers=1).to(dev).eval()
+    with torch.inference_mode():
+        out = pol(env.reset(env.generator(40).to(dev)), env, decode_type="sampling", num_starts=7, seed=3)
+    print("polynet", env_name, "ok", out["reward"].mean().item())
 # 2-opt local search (co_tsp_two_opt): both distance sources, on both sides of the shared-memory residency bound
 # (CO_TWO_OPT_RESIDENT_MAX_NODES = 224); the in-place segment reversal is what racecheck looks at
 for n in (20, 224, 300):
