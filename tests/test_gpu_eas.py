@@ -21,13 +21,16 @@ DEV = torch.device("cuda:0")
 E = 128
 
 
-def _setup(env_name, N, B, seed):
+def _setup(env_name, N, B, seed, use_graph_context=True, **policy_kw):
+    """Seeded policy and instances; `policy_kw` (temperature, tanh_clipping) go to the policy, which `eas_search`
+    reads them from."""
     from rl4co_b200.envs import get_env
     from rl4co_b200.policy import FusedAttentionModelPolicy
 
     torch.manual_seed(seed)
     env = get_env(env_name, generator_params=dict(num_loc=N if env_name == "tsp" else N - 1), check_solution=False)
-    pol = FusedAttentionModelPolicy(env_name=env_name, num_encoder_layers=2)
+    pol = FusedAttentionModelPolicy(env_name=env_name, num_encoder_layers=2, use_graph_context=use_graph_context,
+                                    **policy_kw)
     pol.load_state_dict(name_seeded_weights(pol.state_dict(), seed))
     pol = pol.to(DEV).eval()
     td_host = env.generator(B)
@@ -47,7 +50,7 @@ def _cache(pol, td):
     return hidden, cached, cache, L
 
 
-def _rollout(env_name, pol, td, cached, cache, S, seed, offset=0):
+def _rollout(env_name, pol, td, cached, cache, S, seed, offset=0, tanh_clipping=10.0, temperature=1.0):
     from rl4co_b200 import native
 
     B, N = td["action_mask"].shape
@@ -57,27 +60,29 @@ def _rollout(env_name, pol, td, cached, cache, S, seed, offset=0):
                           td["demand"].contiguous() if vrp else None,
                           td["vehicle_capacity"].reshape(-1).contiguous() if vrp else None, B, N, num_starts=S,
                           forced_start=True, num_loc=N - (1 if vrp else 0), T_max=N if not vrp else 2 * (N - 1),
-                          seed=seed, offset=offset)
+                          seed=seed, offset=offset, tanh_clipping=tanh_clipping, temperature=temperature)
 
 
-def _grad(env_name, td, cached, cache, rows, coef, bad=None):
+def _grad(env_name, td, cached, cache, rows, coef, bad=None, tanh_clipping=10.0, temperature=1.0):
     from rl4co_b200 import native
 
     vrp = env_name == "cvrp"
     return native.eas_key_grad(env_name, cache, rows, coef, graph_ctx=cached.graph_context_or_none,
                                w_capacity=cached.w_capacity, demand=td["demand"].contiguous() if vrp else None,
                                vehicle_capacity=td["vehicle_capacity"].reshape(-1).contiguous() if vrp else None,
-                               bad_rows=bad)
+                               tanh_clipping=tanh_clipping, temperature=temperature, bad_rows=bad)
 
 
-def _oracle_grad(pol, env_name, inst, hidden, L, rows, coef, R):
-    """d(sum_j coef_j ll_j) / dL in float64 through the reference-restated decoder (fixed encoder output)."""
+def _oracle_grad(pol, env_name, inst, hidden, L, rows, coef, R, **kw):
+    """d(sum_j coef_j ll_j) / dL in float64 through the reference-restated decoder (fixed encoder output) -> (the leaf
+    L64 holding it in .grad, the per-step log-probs [rows, T]).  `kw`: temperature, tanh_clipping, use_graph_context
+    of `O.teacher_forced_logprobs`."""
     W64 = O.float64_weights(pol.state_dict(), ())
     L64 = L.detach().double().cpu().requires_grad_(True)
     lp = teacher_forced_logprobs_with_key(W64, env_name, inst, hidden.detach().double().cpu(), rows.cpu(), L64,
-                                          num_starts=R, forced_first=True)
+                                          num_starts=R, forced_first=True, **kw)
     (coef.double().cpu() * lp.sum(1)).sum().backward()
-    return L64
+    return L64, lp.detach()
 
 
 def _samples(env_name, pol, td, cached, cache, S, seed):
@@ -90,8 +95,13 @@ def _samples(env_name, pol, td, cached, cache, S, seed):
     return rows.contiguous(), ll
 
 
-@pytest.mark.parametrize("env_name", ["tsp", "cvrp"])
-@pytest.mark.parametrize("N", [20, 50, 100, 128])
+# the node-slot edges of the SPL = 1 / 2 / 4 instantiations (N = 32, 33, 64, 65), the smallest instance with a choice
+# after the forced start (N = 3) and tsp N = 66; for cvrp N is the mask width, depot included
+GRAD_SIZES = [(n, e) for n in (20, 50, 100, 128) for e in ("tsp", "cvrp")] + \
+    [(n, "tsp") for n in (3, 32, 33, 64, 65, 66)] + [(n, "cvrp") for n in (3, 32, 33, 64, 65)]
+
+
+@pytest.mark.parametrize("N,env_name", GRAD_SIZES)
 @pytest.mark.parametrize("S", [1, 3])
 def test_key_gradient_vs_float64_oracle(env_name, N, S):
     B = 3
@@ -103,7 +113,7 @@ def test_key_gradient_vs_float64_oracle(env_name, N, S):
     torch.testing.assert_close(ll, ll_roll, rtol=1e-5, atol=1e-5)
     dL = torch.matmul(dLf, pol.decoder.pointer.project_out.weight.t())
     inst = {k: td_host[k] for k in td_host.keys()}
-    L64 = _oracle_grad(pol, env_name, inst, hidden, L, rows, coef, S + 1)
+    L64, _ = _oracle_grad(pol, env_name, inst, hidden, L, rows, coef, S + 1)
     rel, zero = O.gradient_errors({"L": dL}, {"L": L64})
     assert not zero and rel["L"] <= 2e-4, rel
 
@@ -149,19 +159,36 @@ def test_infeasible_row_is_reported_and_skipped(env_name):
     torch.testing.assert_close(d, d0, rtol=0, atol=0)
 
 
+# eas_search reads the decoding parameters and the graph context from the policy: settings besides the defaults
+SEARCH_SETTINGS = [(3.0, 0.5, False)]
+
+
 def test_one_iteration_equals_adam_on_the_oracle_gradient():
+    _check_one_iteration_equals_adam(10.0, 1.0, True)
+
+
+@pytest.mark.parametrize("clip,temp,graph_context", SEARCH_SETTINGS)
+def test_one_iteration_equals_adam_at_the_policy_decoding_settings(clip, temp, graph_context):
+    """eas_search passes the policy's tanh clipping, temperature and missing graph context to both of its kernels."""
+    _check_one_iteration_equals_adam(clip, temp, graph_context)
+
+
+def _check_one_iteration_equals_adam(clip, temp, graph_context):
     from rl4co_b200.eas import eas_coefficients, eas_search
     from rl4co_b200.ops import StateAugmentation
 
     B, N, A = 2, 20, 8
-    env, pol, td, _ = _setup("tsp", N, B, seed=21)
+    dec = dict(tanh_clipping=clip, temperature=temp)
+    env, pol, td, _ = _setup("tsp", N, B, seed=21, use_graph_context=graph_context, **dec)
     res = eas_search(pol, env, td, max_iters=1, seed=99, return_logit_key=True)
     tda = StateAugmentation(num_augment=A, augment_fn="dihedral8")(td)
     hidden, cached, cache, L0 = _cache(pol, tda)
+    assert (cached.graph_context_or_none is not None) == graph_context
     S = env.get_num_starts(td)
-    out = _rollout("tsp", pol, tda, cached, cache, S, seed=99, offset=0)
+    out = _rollout("tsp", pol, tda, cached, cache, S, seed=99, offset=0, **dec)
     coef = eas_coefficients(out["reward"].view(S, A, B), "multistart", 0.013, with_incumbent=False)
-    L64 = _oracle_grad(pol, "tsp", {"locs": tda["locs"].cpu()}, hidden, L0, out["actions"], coef, S)
+    L64, _ = _oracle_grad(pol, "tsp", {"locs": tda["locs"].cpu()}, hidden, L0, out["actions"], coef, S,
+                          use_graph_context=graph_context, **dec)
     g64 = L64.grad
     ref = torch.nn.Parameter(L0.detach().double().cpu())
     ref.grad = g64.clone()

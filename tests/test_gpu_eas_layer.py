@@ -12,7 +12,7 @@ import torch
 
 from eas_layer_oracle import teacher_forced_logprobs_with_layer
 from oracle import am_rollout_oracle as O
-from test_gpu_eas import _cache, _setup
+from test_gpu_eas import GRAD_SIZES, SEARCH_SETTINGS, _cache, _setup
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
@@ -38,7 +38,8 @@ def _leaves(packed):
     return {k: v.detach().double().cpu().clone().requires_grad_(True) for k, v in unpack_eas_layer(packed).items()}
 
 
-def _rollout(env_name, td, cached, cache, S, layer, mode=None, seed=0, offset=0, forced=None):
+def _rollout(env_name, td, cached, cache, S, layer, mode=None, seed=0, offset=0, forced=None, tanh_clipping=10.0,
+             temperature=1.0):
     from rl4co_b200 import native
 
     B, N = td["action_mask"].shape
@@ -48,23 +49,25 @@ def _rollout(env_name, td, cached, cache, S, layer, mode=None, seed=0, offset=0,
                           td["locs"].contiguous(), td["demand"].contiguous() if vrp else None,
                           td["vehicle_capacity"].reshape(-1).contiguous() if vrp else None, B, N, num_starts=S,
                           forced_start=True, num_loc=N - (1 if vrp else 0), T_max=N if not vrp else 2 * (N - 1),
-                          seed=seed, offset=offset, forced_actions=forced, layer=layer)
+                          seed=seed, offset=offset, forced_actions=forced, layer=layer, tanh_clipping=tanh_clipping,
+                          temperature=temperature)
 
 
-def _grad(env_name, td, cached, cache, rows, coef, layer, bad=None):
+def _grad(env_name, td, cached, cache, rows, coef, layer, bad=None, tanh_clipping=10.0, temperature=1.0):
     from rl4co_b200 import native
 
     vrp = env_name == "cvrp"
     return native.eas_layer_grad(env_name, cache, rows, coef, layer, graph_ctx=cached.graph_context_or_none,
                                  w_capacity=cached.w_capacity, demand=td["demand"].contiguous() if vrp else None,
                                  vehicle_capacity=td["vehicle_capacity"].reshape(-1).contiguous() if vrp else None,
-                                 bad_rows=bad)
+                                 tanh_clipping=tanh_clipping, temperature=temperature, bad_rows=bad)
 
 
-def _oracle_logprobs(pol, env_name, inst, hidden, rows, leaves, R):
+def _oracle_logprobs(pol, env_name, inst, hidden, rows, leaves, R, **kw):
+    """`kw`: temperature, tanh_clipping, use_graph_context of `O.teacher_forced_logprobs`"""
     W64 = O.float64_weights(pol.state_dict(), ())
     return teacher_forced_logprobs_with_layer(W64, env_name, inst, hidden.detach().double().cpu(), rows.cpu(), leaves,
-                                              num_starts=R, forced_first=True)
+                                              num_starts=R, forced_first=True, **kw)
 
 
 def _samples(env_name, td, cached, cache, S, layer, seed):
@@ -81,8 +84,7 @@ def _flat(grads):
                                         ("W2", slice(E * E + E, 2 * E * E + E)), ("b2", slice(2 * E * E + E, None)))}
 
 
-@pytest.mark.parametrize("env_name", ["tsp", "cvrp"])
-@pytest.mark.parametrize("N", [20, 50, 100, 128])
+@pytest.mark.parametrize("N,env_name", GRAD_SIZES)  # tsp N = 65 / 66: chunk ends on / never on a row end
 @pytest.mark.parametrize("S", [1, 3])
 def test_layer_gradient_vs_float64_oracle(env_name, N, S):
     B = 3
@@ -145,7 +147,8 @@ def test_infeasible_row_is_reported_and_skipped(env_name):
     torch.testing.assert_close(d, d0, rtol=0, atol=0)
 
 
-@pytest.mark.parametrize("env_name,N", [("tsp", 20), ("tsp", 100), ("cvrp", 50), ("cvrp", 128)])
+@pytest.mark.parametrize("env_name,N", [("tsp", 20), ("tsp", 100), ("cvrp", 50), ("cvrp", 128), ("tsp", 32), ("tsp", 33),
+                                        ("tsp", 65), ("cvrp", 33), ("cvrp", 64)])
 def test_rollout_with_layer_vs_oracle(env_name, N):
     from rl4co_b200 import native
 
@@ -181,11 +184,22 @@ def test_rollout_with_layer_vs_oracle(env_name, N):
 
 
 def test_one_iteration_equals_adam_on_the_oracle_gradient():
+    _check_one_iteration_equals_adam(10.0, 1.0, True)
+
+
+@pytest.mark.parametrize("clip,temp,graph_context", SEARCH_SETTINGS)
+def test_one_iteration_equals_adam_at_the_policy_decoding_settings(clip, temp, graph_context):
+    """eas_search passes the policy's tanh clipping, temperature and missing graph context to both of its kernels."""
+    _check_one_iteration_equals_adam(clip, temp, graph_context)
+
+
+def _check_one_iteration_equals_adam(clip, temp, graph_context):
     from rl4co_b200.eas import eas_coefficients, eas_layer_init, eas_search, unpack_eas_layer
     from rl4co_b200.ops import StateAugmentation
 
     B, N, A, lr = 2, 20, 8, 0.0041
-    env, pol, td, _ = _setup("tsp", N, B, seed=21)
+    dec = dict(tanh_clipping=clip, temperature=temp)
+    env, pol, td, _ = _setup("tsp", N, B, seed=21, use_graph_context=graph_context, **dec)
     torch.manual_seed(77)
     res = eas_search(pol, env, td, max_iters=1, seed=99, use_eas_layer=True, use_eas_embedding=False,
                      return_layer=True)
@@ -193,12 +207,14 @@ def test_one_iteration_equals_adam_on_the_oracle_gradient():
     P0 = eas_layer_init(A * B, DEV)
     tda = StateAugmentation(num_augment=A, augment_fn="dihedral8")(td)
     hidden, cached, _, _ = _cache(pol, tda)
+    assert (cached.graph_context_or_none is not None) == graph_context
     cache = cached.rollout_cache.contiguous()  # eas_search's cache: EAS-Lay does not refold the key
     S = env.get_num_starts(td)
-    out = _rollout("tsp", tda, cached, cache, S, P0, seed=99, offset=0)
+    out = _rollout("tsp", tda, cached, cache, S, P0, seed=99, offset=0, **dec)
     coef = eas_coefficients(out["reward"].view(S, A, B), "multistart", 0.013, with_incumbent=False)
     leaves = _leaves(P0)
-    lp = _oracle_logprobs(pol, "tsp", {"locs": tda["locs"].cpu()}, hidden, out["actions"], leaves, S)
+    lp = _oracle_logprobs(pol, "tsp", {"locs": tda["locs"].cpu()}, hidden, out["actions"], leaves, S,
+                          use_graph_context=graph_context, **dec)
     (coef.double().cpu() * lp.sum(1)).sum().backward()
     for k, leaf in leaves.items():
         ref = torch.nn.Parameter(leaf.detach().clone())

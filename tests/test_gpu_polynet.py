@@ -40,8 +40,9 @@ def _w64(pol):
     return O.float64_weights(pol.state_dict(), ())
 
 
-def _oracle_steps(W64, env_name, inst, h64, acts, S, strategy=None):
-    """Teacher-forced float64 log-probs of `acts` and, per step, the oracle's full log-prob row."""
+def _recorded_steps(teacher_forced, *args, **kw):
+    """`teacher_forced(*args, **kw)` (an `O.teacher_forced_logprobs` variant) -> its float64 log-probs and, per decoder
+    step, the oracle's full log-prob row."""
     rows = []
     real = O.process_logits
 
@@ -52,11 +53,17 @@ def _oracle_steps(W64, env_name, inst, h64, acts, S, strategy=None):
 
     O.process_logits = recording
     try:
-        lp = teacher_forced_logprobs_polynet(W64, env_name, inst, h64, acts, num_starts=S, forced_first=True,
-                                             strategy=strategy)
+        lp = teacher_forced(*args, **kw)
     finally:
         O.process_logits = real
     return lp.detach(), torch.stack(rows, 1)  # [R, T], [R, T - 1, N]
+
+
+def _oracle_steps(W64, env_name, inst, h64, acts, S, strategy=None, **kw):
+    """Teacher-forced float64 log-probs of `acts` and, per step, the oracle's full log-prob row.  `kw`: temperature,
+    tanh_clipping, use_graph_context of `O.teacher_forced_logprobs`."""
+    return _recorded_steps(teacher_forced_logprobs_polynet, W64, env_name, inst, h64, acts, num_starts=S,
+                           forced_first=True, strategy=strategy, **kw)
 
 
 def _check_greedy(lp_gpu, acts, lp64, full64):
@@ -71,8 +78,9 @@ def _check_greedy(lp_gpu, acts, lp64, full64):
 SIZES = [(1, 2), (1, 5), (3, 2), (3, 3), (3, 9), (128, 2), (128, 128), (128, 259)]
 
 
-@pytest.mark.parametrize("k,S", SIZES)
-@pytest.mark.parametrize("N", [20, 50, 100, 128])
+# plus the node-slot edges of the SPL = 1 / 2 / 4 instantiations at one (k, S)
+@pytest.mark.parametrize("N,k,S", [(n, k, s) for n in (20, 50, 100, 128) for k, s in SIZES] +
+                         [(n, 3, 9) for n in (32, 33, 64, 65)])
 @pytest.mark.parametrize("env_name", ["tsp", "cvrp"])
 def test_fused_greedy_vs_oracle(env_name, N, k, S):
     env, pol, td, inst = _setup(env_name, N, 2, k, seed=N + k + S)

@@ -218,8 +218,9 @@ def _slice_call(a, k, b0, b1, S):
             a[i] = a[i][b0:b1].contiguous()
     a[9] = b1 - b0
     k = dict(k)
-    if k.get("node_limit") is not None:
-        k["node_limit"] = k["node_limit"][b0:b1].contiguous()
+    for key in ("node_limit", "layer"):  # op / pctsp limits, the EAS-Lay layer: one row per instance
+        if k.get(key) is not None:
+            k[key] = k[key][b0:b1].contiguous()
     if k.get("forced_actions") is not None:
         k["forced_actions"] = k["forced_actions"][rows].contiguous()
     if k.get("noise") is not None:
